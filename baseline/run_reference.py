@@ -27,12 +27,12 @@ def _unavailable(why):
 
 def run(args):
     if not os.path.isdir(os.path.join(REF, "dear")):
-        src = "/root/reference"
-        if os.path.isdir(os.path.join(src, "dear")):
+        src = os.environ.get("DEAR_REFERENCE_DIR", "")
+        if src and os.path.isdir(os.path.join(src, "dear")):
             import shutil
             shutil.copytree(src, REF, dirs_exist_ok=True)
         else:
-            return _unavailable("baseline/_ref is missing and /root/reference is not mounted "
+            return _unavailable("baseline/_ref is missing and DEAR_REFERENCE_DIR does not name a checkout of the reference "
                                 "(the reference has no setup.py; comm_core needs MPI)")
     try:
         import torch

@@ -25,6 +25,7 @@ if ROOT not in sys.path:
 
 BASELINE_PUBLISHED = None   # the reference publishes no throughput number (BASELINE.md §1)
 BERT_MODELS = ("bert", "bert_large", "bert_base")
+DUMP_PARAM_SAMPLE = 1 << 22        # 16 MB of float32: the parameter sample written by --dump-outputs
 
 
 def parse_args(argv=None):
@@ -43,15 +44,14 @@ def parse_args(argv=None):
     ap.add_argument("--overlap-update", type=int, default=(int(os.environ["DEAR_BENCH_OVERLAP"]) if "DEAR_BENCH_OVERLAP" in os.environ else None),
                     help="graph mode: capture step(previous gradients) -> forward -> backward so the update + all-gather "
                          "kernels overlap the forward inside the graph (utils/train.py) -- DeAR's defining overlap; default: on "
-                         "with peers and for BERT (+3.5 %% on one B200), off for a CNN on a single GPU (nothing to hide; "
-                         "the natural body measured faster there)")
+                         "with peers and for BERT, off for a CNN on a single GPU (nothing to hide there)")
     ap.add_argument("--fused-bn", type=int, default=int(os.environ.get("DEAR_BENCH_FUSED_BN", "1")),
                     help="ResNets: fused channels-last BatchNorm(+add)+ReLU kernels (csrc/bn_act.cu)")
     ap.add_argument("--fused-ln", type=int, default=int(os.environ.get("DEAR_BENCH_FUSED_LN", "1")),
                     help="BERT: dropout + add + LayerNorm in one kernel (csrc/ln_fused.cu)")
     ap.add_argument("--tc-ffn", type=int, default=int(os.environ.get("DEAR_BENCH_TC_FFN", "0")),
-                    help="BERT bf16: feed-forward block on the hand-written tcgen05 GEMMs with fused GELU epilogues (csrc/tc_ffn_hw.cu); "
-                         "off by default: cuBLAS + the fused bias/GELU kernels are faster (profiles/README.md R2.5)")
+                    help="BERT bf16: feed-forward block on the hand-written wgmma GEMMs with fused GELU epilogues (csrc/tc_ffn_hw.cu); "
+                         "off by default: cuBLAS + the fused bias/GELU kernels of csrc/ln_fused.cu")
     ap.add_argument("--threshold", type=float, default=25.0)
     ap.add_argument("--momentum", type=float, default=0.0)
     ap.add_argument("--optimizer", choices=["sgd", "adam", "adamw"], default="sgd",
@@ -62,7 +62,14 @@ def parse_args(argv=None):
                     help="end-to-end run: spin this long on the copy stream before each prefetch upload so the PCIe DMA does "
                          "not start at the step boundary, where the rotated step runs the update + all-gather kernels "
                          "(utils/data.py). Default: 2000 with --overlap-update 1, else 0")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy: the loss and a "
+                         "fixed, seeded sample of the parameters (float32, at most %d values).  Runs with deterministic "
+                         "cuDNN algorithms instead of autotuned ones, so that every run computes the same bits (slower)"
+                         % DUMP_PARAM_SAMPLE)
     args = ap.parse_args(argv)
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs is only implemented for --impl dear")
     is_bert = args.model in BERT_MODELS
     if args.batch_size is None:
         args.batch_size = 32 if is_bert else 64
@@ -70,10 +77,8 @@ def parse_args(argv=None):
         # BERT-large is specified in bf16 (BASELINE.json); ResNet-50 runs at the reference's precision
         args.dtype = "bf16" if is_bert else "fp32"
     if args.overlap_update is None:
-        # Rotated body wherever it measured faster: with peers (it hides the all-gather tail: ResNet-50 13.51 -> 13.38 ms
-        # at 8 GPUs) and for BERT even on one GPU (+3.5 %).  A CNN on ONE GPU has no communication to hide and the
-        # natural body is faster there (ResNet-50 13.25 vs 13.27 ms resident, 13.26 vs 13.44 ms end to end; VGG-16
-        # 21.12 (round-1 eager loop, natural order) vs 21.45 ms), so that case keeps it.
+        # Rotated body with peers (the update + all-gather kernels overlap the next forward) and for BERT; a CNN on ONE
+        # GPU has no communication to hide, so that case keeps the natural body.
         args.overlap_update = 1 if (is_bert or int(os.environ.get("WORLD_SIZE", "1")) > 1) else 0
     return args
 
@@ -177,7 +182,14 @@ def run_dear(args):
     rank, world = dear.rank(), dear.size()
     device = dear.device()
     cuda = device.type == "cuda"
-    torch.backends.cudnn.benchmark = True
+    if args.dump_outputs:
+        # dumps are for comparing builds output for output, so the same arguments must compute the same bits on every
+        # run: autotuning picks convolution algorithms by timing, and some of them accumulate with atomics.  Slower
+        # than the autotuned default; the throughput of a dumping run is not the headline number.
+        torch.backends.cudnn.benchmark = False
+        torch.backends.cudnn.deterministic = True
+    else:
+        torch.backends.cudnn.benchmark = True
     torch.manual_seed(1234)
 
     wl = Workload(args, device, rank)
@@ -246,8 +258,14 @@ def run_dear(args):
 
     sampler = ClockSampler(device.index if cuda else 0).start() if (cuda and rank == 0) else None
     wall0 = time.time()
-    ms, launches = timed(lambda: step(*dev_batch), args.steps)
+    last_loss = [None]
+
+    def timed_step():
+        last_loss[0] = step(*dev_batch)
+    ms, launches = timed(timed_step, args.steps)
     wall1 = time.time()
+    if args.dump_outputs and rank == 0:
+        _dump_outputs(args.dump_outputs, last_loss[0], model)
     if args.graph and cuda:
         launches = int(round(per_step_launches * args.steps))
 
@@ -292,9 +310,9 @@ def run_dear(args):
                "optimizer": "%s lr=%g" % (args.optimizer.upper(), lr), "threshold_mb": args.threshold, "buckets": len(opt.engine.plan.buckets),
                "params": n_params, "backend": dear.backend(), "cuda_graph": bool(step.use_graph),
                "update_overlaps_forward_in_graph": bool(step.overlap_update),
-               "l2": "no explicit flush: each step streams activations+weights far larger than the 126 MB L2"}
+               "l2": "no explicit flush: each step streams activations+weights far larger than the 50 MB L2"}
         if wl.is_bert:
-            cfg.update(seq_len=args.sentence_len, fused_dropout_add_ln=wl.fused_ln, tcgen05_ffn=wl.tc_ffn)
+            cfg.update(seq_len=args.sentence_len, fused_dropout_add_ln=wl.fused_ln, wgmma_ffn=wl.tc_ffn)
         else:
             cfg.update(image=wl.image, channels_last=bool(args.channels_last), fused_bn_relu=getattr(wl, "fused_bn", False))
         out = {
@@ -314,6 +332,22 @@ def run_dear(args):
         traceback.print_exc()
     dear.shutdown()
     return 0
+
+
+def _dump_outputs(out_dir, loss, model):
+    """The last timed step's loss and a seeded sample of the parameters as they stand after it (before the end-to-end
+    run moves them further): two builds run with the same arguments can be compared output for output."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().cpu().reshape(1).numpy())
+    flat = torch.cat([p.detach().reshape(-1).float() for p in model.parameters()])
+    n = flat.numel()
+    if n > DUMP_PARAM_SAMPLE:
+        g = torch.Generator().manual_seed(0)
+        idx = torch.randint(0, n, (DUMP_PARAM_SAMPLE,), generator=g).sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(out_dir, "params_sample.npy"), flat.cpu().numpy())
 
 
 def _max_over_ranks(v, world):

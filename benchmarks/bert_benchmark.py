@@ -24,7 +24,7 @@ def main(argv=None):
     ap.add_argument("--lr", type=float, default=2e-5)
     ap.add_argument("--config", type=str, default=None, help="optional JSON file with BertConfig fields")
     ap.add_argument("--fused-ln", type=int, default=1, help="dropout + add + LayerNorm in one kernel (CUDA)")
-    ap.add_argument("--tc-ffn", type=int, default=0, help="feed-forward block on the tcgen05 GEMMs (CUDA, bf16; opt-in)")
+    ap.add_argument("--tc-ffn", type=int, default=0, help="feed-forward block on the wgmma GEMMs (CUDA, bf16; opt-in)")
     common.add_common_args(ap)
     args = ap.parse_args(argv)
     method, cuda = common.init_runtime(args)

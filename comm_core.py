@@ -7,7 +7,7 @@
 
 ``Communicator`` is :class:`dear_pytorch_b200.parallel.comm.Comm`: the same method names (``bcast, reduce, allReduce,
 allReduceRB, allReduceRSAG, reduceScatter, allGather, multiBcast, sendrecv, synchronize, barrier, syncStream,
-getNumOfFreeStreams, destroy, reload``) on the fused sm_100a kernels of ``dear_pytorch_b200._C`` (or on
+getNumOfFreeStreams, destroy, reload``) on the fused sm_90a kernels of ``dear_pytorch_b200._C`` (or on
 torch.distributed for the gloo / nccl backends).  ``barriar`` keeps the reference's spelling.
 """
 from dear_pytorch_b200 import init, rank, size, barrier  # noqa: F401

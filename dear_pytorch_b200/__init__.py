@@ -1,4 +1,4 @@
-"""dear_pytorch_b200 — a B200-native DeAR (decoupled all-reduce) data-parallel engine.
+"""dear_pytorch_b200 — an H100-native DeAR (decoupled all-reduce) data-parallel engine.
 
 Public API (same surface as the reference package ``dear``, dear/__init__.py:3-9)::
 

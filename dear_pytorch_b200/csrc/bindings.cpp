@@ -3,7 +3,7 @@
 // Counterpart of the reference's `comm_core` module
 // (common/comm_core/src/comm_core.cpp:12-37): same operation family, but
 // process bootstrap comes from torch.distributed's store (no MPI) and the data
-// path is our own sm_100a kernels (no NCCL).
+// path is our own sm_90a kernels (no NCCL).
 #include <torch/extension.h>
 #include <torch/csrc/distributed/c10d/Store.hpp>
 
@@ -39,7 +39,7 @@ std::vector<torch::Tensor> bias_gelu_backward(const torch::Tensor& dh, const tor
 } }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "B200-native DeAR communication runtime (fused reduce-scatter / SGD+all-gather kernels)";
+  m.doc() = "H100-native DeAR communication runtime (fused reduce-scatter / SGD+all-gather kernels)";
 
   m.attr("MAX_RANKS") = kMaxRanks;
   m.attr("PROVIDER_HOST_SHM") = static_cast<int>(Provider::HOST_SHM);

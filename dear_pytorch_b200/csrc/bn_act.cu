@@ -1,8 +1,7 @@
 // bn_act.cu — fused BatchNorm2d (+ residual add) (+ ReLU), channels-last, training and inference.
 //
-// Why: a steady-state ncu launch list of the ResNet-50 step (profiles/README.md) shows cuDNN
-// BatchNorm forward/backward plus the separate ReLU / add elementwise kernels at ~51 % of GPU
-// kernel time — all of it HBM-bound.  Unfused, a BN+ReLU layer costs ~13 tensor passes per
+// Why: in the ResNet-50 step, cuDNN BatchNorm forward/backward plus the separate ReLU / add elementwise kernels
+// are a large share of GPU kernel time — all of it HBM-bound.  Unfused, a BN+ReLU layer costs ~13 tensor passes per
 // iteration (BN fwd 3, ReLU fwd 2, ReLU bwd 3, BN bwd 5); fused it costs 8:
 //     forward : stats (read x) -> finalize -> apply (read x [,z], write y)
 //     backward: reduce (read dy, x [,y]) -> finalize -> apply (read dy, x [,y], write dx [,dz])
@@ -20,6 +19,7 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <torch/extension.h>
+#include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAStream.h>
 #include <c10/cuda/CUDAGuard.h>
 
@@ -409,7 +409,8 @@ static bool make_geo(int64_t M, int64_t C, int vec, Geo* g) {
   g->ty = kThreads / txv;
   g->ch_groups = static_cast<int>(cv / txv);
   int64_t want = (M + int64_t(g->ty) * 8 - 1) / (int64_t(g->ty) * 8);    // >= 8 rows per thread
-  int64_t cap = std::max<int64_t>(1, (148 * 8) / g->ch_groups);      // 8 x 256 threads per SM
+  const int64_t sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  int64_t cap = std::max<int64_t>(1, (sms * 8) / g->ch_groups);      // 8 x 256 threads per SM
   g->row_blocks = static_cast<int>(std::max<int64_t>(1, std::min(want, cap)));
   return true;
 }

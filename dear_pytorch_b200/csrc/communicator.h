@@ -1,6 +1,6 @@
 // communicator.h — native communication runtime of the DeAR engine.
 //
-// `Communicator` is the B200 counterpart of the reference's NCCL+MPI
+// `Communicator` is the H100 counterpart of the reference's NCCL+MPI
 // `Communicator` class (common/comm_core/src/communicator.h:52-96): it owns the
 // communication streams/events and exposes the same family of operations
 // (bcast, reduce, allReduce, allReduceRB, allReduceRSAG, reduceScatter,
@@ -40,11 +40,9 @@ struct CommOptions {
   // Kernel A variant per bucket: -1 = pick by bucket size (one-shot below `pipe_min_bytes`, stripe-pipelined TMA
   // pull above, NVLS ld_reduce only on request); 0 / 1 / 2 force RS_ALGO_ONESHOT / _PIPE / _NVLS for every bucket.
   int rs_algo = -1;
-  int64_t pipe_min_bytes = int64_t(1) << 60;   // auto never picks the pipelined variant unless this is lowered:
-                                               // at 8 GPUs the one-shot kernel on a wide grid is faster at every
-                                               // size (profiles/r2/session_8gpu_a.log)
+  int64_t pipe_min_bytes = int64_t(1) << 60;   // auto never picks the pipelined variant unless this is lowered
   int rs_grid_big = 128;                       // CTA bound for buckets >= big_bucket_bytes (their pack phase scales
-  int64_t big_bucket_bytes = 128ll << 20;      // with the CTA count: 846 / 711 us at 32 / 96 CTAs for 392 MB, P=8)
+  int64_t big_bucket_bytes = 128ll << 20;      // with the CTA count)
   int64_t stripe_target_bytes = 8ll << 20;   // bucket bytes per stripe the pipelined kernel aims for
   bool separate_ag_stream = true;            // all-gathers on their own stream (reference: three communicators)
 };

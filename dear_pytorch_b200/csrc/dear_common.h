@@ -1,6 +1,6 @@
-// dear_common.h — shared declarations for the B200-native DeAR runtime.
+// dear_common.h — shared declarations for the H100-native DeAR runtime.
 //
-// Everything in this header is usable from host C++ and from sm_100a device
+// Everything in this header is usable from host C++ and from sm_90a device
 // code: the host-emulation backend (emu.cpp, used for CPU/gloo plumbing
 // tests) and the CUDA kernels (kernels.cu) share the SAME argument structs
 // and the SAME per-element math, so a CPU test of the emulation backend
@@ -25,7 +25,7 @@
 
 namespace dear {
 
-constexpr int kMaxRanks = 16;            // one NVSwitch domain (8 on HGX B200)
+constexpr int kMaxRanks = 16;            // one NVSwitch domain (8 on HGX H100)
 constexpr int kNumChannels = 4096;       // signal-pad channels per arena
 constexpr int kChannelsPerBucket = 4;    // RS_READY, RS_DONE, AG_ARRIVE, AG_PUSHED
 constexpr int kGeneralChannels = 64;     // channels [0,64) are for general ops

@@ -37,10 +37,9 @@ __device__ __forceinline__ uint4 ld_stream(const void* p) {
                : "memory");
   return v;
 }
-// 128-bit load of PEER memory.  Peer addresses bypass the local L2 and are cached in L1 only; measured on 2 B200s
-// (profiles/r2/p2p_probe_2gpu.log) the allocating form sustains ~6 % more NVLink read bandwidth than
-// L1::no_allocate (646 vs 611 GB/s per direction at 64 CTAs).  Every peer address is read once per kernel and L1
-// is invalidated at kernel boundaries, so there is no staleness to worry about.
+// 128-bit load of PEER memory.  Peer addresses bypass the local L2 and are cached in L1 only (the allocating form is
+// used rather than L1::no_allocate; tools/p2p_probe.cu compares the two).  Every peer address is read once per kernel
+// and L1 is invalidated at kernel boundaries, so there is no staleness to worry about.
 __device__ __forceinline__ uint4 ld_peer(const void* p) {
   uint4 v;
   asm volatile("ld.global.v4.u32 {%0,%1,%2,%3}, [%4];"

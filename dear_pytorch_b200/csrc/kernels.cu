@@ -1,4 +1,4 @@
-// kernels.cu — sm_100a device code of the DeAR runtime.
+// kernels.cu — sm_90a device code of the DeAR runtime.
 //
 // Kernel A (rs_kernel):   gradient pack + reduce-scatter + fp32 accumulate + 1/P scale
 //                         replaces: bucket copy_ (dear/dear_dopt.py:265), ncclReduceScatter

@@ -1,12 +1,11 @@
-// rs_pipe.cu — Kernel A, stripe-pipelined variant (sm_100a): gradient pack + reduce-scatter + fp32
+// rs_pipe.cu — Kernel A, stripe-pipelined variant (sm_90a): gradient pack + reduce-scatter + fp32
 // accumulate + 1/P scale for buckets that are bandwidth-bound (>= a few MB).
 //
 // Replaces, like the one-shot rs_kernel in kernels.cu: the per-parameter bucket copy_
 // (dear/dear_dopt.py:265), ncclReduceScatter (common/comm_core/src/communicator.cpp:157-169) and div_ (:306).
 //
 // Why a second variant.  The one-shot kernel packs the WHOLE bucket, crosses one flag round and then pulls:
-// for a 392 MB bucket at P=2 the pack was 395 us of 741 us, at P=8 135 us of 740 us (round-1 profile) — NVLink
-// idles while HBM copies and vice versa.  Here the shard is cut into stripes; stripe k of every shard is packed
+// for a large bucket the pack is a large fraction of the kernel — NVLink idles while HBM copies and vice versa.  Here the shard is cut into stripes; stripe k of every shard is packed
 // and published while stripe k-1 is being pulled, and the pull itself is moved off the LSU:
 //
 //   warps 7-18  PACK      copy this rank's gradients into the symmetric bucket, stripe-major, from a host-built work
@@ -18,8 +17,7 @@
 //   warps 1-6   REDUCE    accumulate the P slots of a chunk in fp32 registers (fixed peer order => run-to-run
 //                         deterministic), scale by 1/P, write the fp32 shard
 //
-// Measured basis (tools/p2p_probe.cu, profiles/r2/p2p_probe_2gpu.log): bulk-copy pulls reach the NVLink
-// plateau (644 GB/s per direction, both directions loaded) with 32 CTAs where 128-bit register loads need 64,
+// Bulk-copy pulls (tools/p2p_probe.cu compares them with 128-bit register loads) need fewer CTAs to keep NVLink busy,
 // and they leave the CTA's threads free to run the pack concurrently.
 #include <cuda_runtime.h>
 #include <stdexcept>

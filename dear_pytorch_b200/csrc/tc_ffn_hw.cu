@@ -1,31 +1,20 @@
-// tc_ffn_hw.cu — hand-written tcgen05 GEMMs for the transformer FFN with a TWO-WARPGROUP epilogue.
+// tc_ffn_hw.cu — hand-written Hopper (sm_90a) wgmma GEMMs for the transformer FFN with the GELU in the epilogue.
 //
 //     ffn_up_hw    : H = gelu(Z),  Z = X W^T + b      X [M,K], W [N,K], b [N]  (bf16, fp32 accumulate)  ->  H, Z [M,N]
 //     ffn_dgelu_hw : dZ = (dY Wt^T) * gelu'(Z)        dY [M,K], Wt [N,K] (= transposed down-projection weight), Z [M,N]
-//   (one kernel template, two epilogue modes; both operands K-major)
+//   (one kernel template, two epilogue modes; A is K-major, B is K-major or MN-major)
 //
-// Why this kernel exists: the CUTLASS-collective variants of round 1 (removed from the tree since) ran the same op but were
-// epilogue-issue-bound — ncu (profiles/prof_bert_ops_summary.md) shows the tensor pipe falling from 59 %
-// to 28 % when the GELU moves into the epilogue, because their 4 epilogue warps (one per SM sub-partition)
-// cannot hide the MUFU/FMA latency of 16 k erf-GELUs per tile.  Here the epilogue has 8 warps: warps w and
-// w+4 share TMEM lane quadrant w%4 (the hardware restricts a warp to lanes 32*(warp%4)..+31) and split the
-// tile's 256 accumulator columns in halves, so every sub-partition has two resident epilogue warps.
+// Why this kernel exists: a library GEMM followed by a GELU kernel writes the [tokens, 4*hidden] pre-activation, reads it
+// back and writes the activation; here the epilogue applies bias + GELU (or GELU') to the accumulators before the one
+// store, and the dgrad reads the down-projection weight as nn.Linear stores it.
 //
-// Structure (one CTA per SM, persistent over 128x256 output tiles, K step 64):
-//   warp 0      TMA producer: cp.async.bulk.tensor.2d (128B swizzle) A 128x64 + B 256x64 into a 4-stage ring,
-//               mbarrier expect_tx / complete_tx
-//   warp 1      MMA issuer: one thread issues tcgen05.mma.cta_group::1.kind::f16 (M128 N256 K16) x4 per stage,
-//               tcgen05.commit -> "stage empty" barrier, and -> "accumulator full" barrier after the last K step
-//   warp 2      allocates / frees the 512 TMEM columns (2 accumulator stages x 256 fp32 columns)
-//   warps 4-11  epilogue: tcgen05.ld 32x32b.x32 -> +bias -> erf-GELU -> 16-byte-vector global stores (H, Z); arrive on
-//               "accumulator empty" so the MMA warp can start tile i+2 while tile i drains
-//
-// STATUS: validated on B200 (tests/test_tc_gemm.py::test_handwritten_*, fp32 oracle; 1/2/4-CTA multicast clusters, K-major
-// and MN-major B).  Measured (profiles/r2/bert_ops_bench_r2_final.json): up+GELU 27.6 us and dgrad x GELU' 28.5 us (on the
-// weight as stored) against 25.3 / 29.5 us for cuBLAS + elementwise kernels; multicast clusters of 2 / 4 change nothing
-// (27.8 / 28.4 us): the operand traffic is not the limiter.  ncu (prof_tc_ffn_hw_cl1_summary.md): tensor
-// pipe 29 % active — two serialized ~10 us epilogues per CTA (256 tiles on 148 SMs), not the mainloop, set the pace.  The
-// kernel is opt-in (bench.py --tc-ffn 1, BertConfig tc_ffn); the default FFN stays cuBLAS + the fused bias/GELU kernels of ln_fused.cu.
+// Structure (one CTA per SM, persistent over 128x128 output tiles, K step 64):
+//   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor.2d (128B swizzle) A 128x64 + B 128x64 into a
+//                   6-stage ring, mbarrier expect_tx / complete_tx.  It runs ahead into the next tile while the
+//                   consumers are in their epilogue, so loads and the GELU math overlap.
+//   warpgroups 1-2  consumers: each owns 64 rows of the tile and issues wgmma.mma_async m64n128k16 (bf16 in shared
+//                   memory, fp32 accumulators in registers) x4 per stage; every warp releases the stage with one
+//                   mbarrier arrive.  Epilogue straight from the accumulator registers: +bias -> erf-GELU -> bf16 stores.
 // Every mbarrier wait is bounded and traps instead of spinning forever.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -43,15 +32,15 @@ void count_launch();
 
 namespace hw {
 
-constexpr int kTileM = 128, kTileN = 256, kTileK = 64, kUmmaK = 16;
-constexpr int kStages = 4, kAccStages = 2;
+constexpr int kTileM = 128, kTileN = 128, kTileK = 64, kWgmmaK = 16;
+constexpr int kStages = 6;
 constexpr int kABytes = kTileM * kTileK * 2;            // 16 KB
-constexpr int kBBytes = kTileN * kTileK * 2;            // 32 KB
-constexpr int kStageBytes = kABytes + kBBytes;          // 48 KB
-constexpr int kNumThreads = 384;                        // 12 warps
-constexpr int kEpilogueWarp0 = 4, kEpilogueWarps = 8;
-constexpr int kTmemCols = kAccStages * kTileN;          // 512
+constexpr int kBBytes = kTileN * kTileK * 2;            // 16 KB
+constexpr int kStageBytes = kABytes + kBBytes;          // 32 KB
+constexpr int kNumThreads = 384;                        // 3 warpgroups: producer + 2 consumers
+constexpr int kConsumerWarps = 8;
 constexpr int kSmemBytes = kStages * kStageBytes + 1024 /* alignment slack */ + 256 /* barriers */;
+static_assert(kSmemBytes <= 227 * 1024, "shared memory ring exceeds the 227 KB a block may use");
 
 // ---------------------------------------------------------------------------------------------- PTX
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -64,6 +53,15 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// arrive on the barrier at the same shared-memory offset in CTA `cta` of this cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 remote;\n\t"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [remote];\n\t}"
+      ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -91,8 +89,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
   asm volatile(
@@ -120,81 +116,54 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma
+__device__ __forceinline__ void fence_accumulators(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem]; accumulate == 0 overwrites the accumulator
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64x128, registers] += A[64x16, smem] * B[16x128, smem]; TRANS_B = 1: B is MN-major (n contiguous)
+template <int TRANS_B>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "
+      "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, 1, 1, 1, 0, %66;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "n"(TRANS_B)
       : "memory");
 }
-// all previously issued tcgen05.mma of this thread arrive on the mbarrier when they complete
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// ... and on the barrier at the same offset in every CTA of `mask` (a stage that a peer's multicast load will overwrite)
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout), K-major operand, 128-byte swizzle:
-//   [0,14) start address >> 4   [16,30) leading byte offset >> 4 (=1: unused for swizzled K-major)
-//   [32,46) stride byte offset >> 4 (8 rows x 128 B = 1024 B between 8-row groups)   [46,48) version = 1 (sm_100)
-//   [49,52) base offset = 0 (tiles are 1024-byte aligned)   [61,64) layout type = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
+// wgmma shared-memory matrix descriptor, 128-byte swizzle:
+//   [0,14) start address >> 4   [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4
+//   [49,52) base offset = 0 (tiles are 1024-byte aligned)   [62,64) layout type = 1 (SWIZZLE_128B)
+// K-major operand: rows of 64 bf16 (128 bytes), SBO = 1024 B between 8-row groups, LBO unused.
+// MN-major operand (B[n][k] = W[k][n] for a row-major W [K, N]): canonical layout in 16-byte units
+// ((8,n),(8,k)) : ((1,LBO),(8,SBO)) — an atom is 8 k-rows of 128 bytes (64 contiguous n); LBO = distance between 64-wide
+// n blocks, SBO = distance between 8-row k groups.  A stage holds kTileN/64 blocks of {64 n, kTileK k} = 8 KB each, so
+// LBO = 8192 B and SBO = 1024 B.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(lbo >> 4) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// MN-major operand (the matrix is stored with its M/N index contiguous, e.g. B[n][k] = W[k][n] for a row-major W
-// [K, N]), 128-byte swizzle.  Canonical layout in 16-byte units: ((8,n),(8,k)) : ((1,LBO),(8,SBO)) — an atom is 8
-// k-rows of 128 bytes (64 contiguous n); LBO = distance between 64-wide n blocks, SBO = distance between 8-row k groups.
-// Our stage holds kTileN/64 TMA boxes of {64 n, kTileK k} = 8 KB each, so LBO = 8192 B and SBO = 1024 B.
-__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((kTileK * 128) >> 4) << 16;     // LBO: next 64-wide n block
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;               // SBO: next group of 8 k rows
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): [4,6) D format = 1 (f32), [7,10) A format = 1 (bf16),
-// [10,13) B format = 1 (bf16), bit 15 / 16 A / B major = 0 (K-major), [17,23) N >> 3, [24,29) M >> 4
-constexpr uint32_t kInstrDesc = (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(kTileN >> 3) << 17) |
-                                (static_cast<uint32_t>(kTileM >> 4) << 24);
-constexpr uint32_t kInstrDescBMN = kInstrDesc | (1u << 16);            // B operand MN-major
 
 // ------------------------------------------------------------------------------------------ GELU
 // Phi(-|x|) by Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7): 2 MUFU + ~12 FMA per element
@@ -235,13 +204,21 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
 // MODE_DGELU: aux = Z [M,N] (read); out0 = dZ = acc * gelu'(Z),  out1 unused
 enum EpilogueMode { MODE_UP = 0, MODE_DGELU = 1 };
 
+// B operand of the MN-major path split into pieces of {64 n, kPieceK k}: enough pieces that every CTA of a cluster
+// loads (and multicasts) the same number
+template <int CL>
+struct BmnPieces {
+  static constexpr int kNBlocks = kTileN / 64;
+  static constexpr int kCount = kNBlocks > CL ? kNBlocks : CL;
+  static constexpr int kPerBlock = kCount / kNBlocks;
+  static constexpr int kRowsK = kTileK / kPerBlock;
+};
+
 // BMN: the B operand is given as a row-major [K, N] matrix (MN-major) instead of [N, K] (K-major): the dgrad GEMM
 // dH = dY W2 reads the nn.Linear weight W2 [hidden, inter] as it is stored — no transposed copy per step.
 // CL: CTAs per cluster (1, 2 or 4).  The CTAs of a cluster work on vertically adjacent output tiles (same n range); each
-// loads 1/CL of the B tile and MULTICASTS it to all of them, so per K step a CTA makes L2 serve 16 + 32/CL KB instead of
-// 48 KB.  Why: ncu on the CL = 1 kernel (profiles/r2/prof_tc_ffn_hw_cl1_summary.md) shows the tensor pipe 29 % active
-// and 201 MB of L2->SM traffic in 30 us = 6.7 TB/s, which IS the chip's L2 throughput cap (~6300 B/clk, B300_MICROARCH.md):
-// a 128x256 tile per CTA re-reads B 16 times and A 16 times.  Multicast is the B200 answer: one L2 read, CL deliveries.
+// loads 1/CL of the B tile and MULTICASTS it to all of them, so per K step a CTA makes L2 serve 16 + 16/CL KB instead of
+// 32 KB.
 template <int MODE, bool BMN, int CL>
 __global__ void __launch_bounds__(kNumThreads, 1)
 ffn_hw_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
@@ -250,13 +227,10 @@ ffn_hw_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant_
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
-  uint64_t* full_bar = bars;                             // [kStages]   TMA -> MMA
-  uint64_t* empty_bar = bars + kStages;                  // [kStages]   MMA -> TMA
-  uint64_t* acc_full_bar = bars + 2 * kStages;           // [kAccStages] MMA -> epilogue
-  uint64_t* acc_empty_bar = acc_full_bar + kAccStages;   // [kAccStages] epilogue -> MMA
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(acc_empty_bar + kAccStages);
+  uint64_t* full_bar = bars;                             // [kStages]   TMA -> consumers
+  uint64_t* empty_bar = bars + kStages;                  // [kStages]   consumers (of every CTA in the cluster) -> TMA
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   const int tiles_m = (M + kTileM - 1) / kTileM, tiles_n = (N + kTileN - 1) / kTileN;
   const int num_kb = (K + kTileK - 1) / kTileK;
   // cluster-tile schedule: cluster c takes every (gridDim/CL)-th group of CL vertically adjacent tiles
@@ -266,25 +240,18 @@ ffn_hw_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant_
   const int num_ct = tiles_mc * tiles_n;
   constexpr uint16_t kAllCtas = static_cast<uint16_t>((1u << CL) - 1);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CL); }
-    for (int a = 0; a < kAccStages; ++a) { mbar_init(&acc_full_bar[a], 1); mbar_init(&acc_empty_bar[a], kEpilogueWarps); }
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps * CL); }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_base_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  if (CL > 1) cluster_sync_all();                        // the peer's barriers exist before anything signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
+  if (CL > 1) cluster_sync_all();                        // the peers' barriers exist before anything signals them
 
-  if (warp == 0) {
-    // ===================================================================== TMA producer (one lane)
-    if (lane == 0) {
+  if (wg == 0) {
+    // ===================================================================== TMA producer (one thread)
+    if (threadIdx.x == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int ct = cid; ct < num_ct; ct += ncl) {
         const int m0 = ((ct % tiles_mc) * CL + crank) * kTileM, n0 = (ct / tiles_mc) * kTileN;
@@ -294,14 +261,14 @@ ffn_hw_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant_
           uint8_t* a_dst = smem + stage * kStageBytes;
           tma_load_2d(a_dst, &tmap_a, &full_bar[stage], kb * kTileK, m0);
           if (BMN) {
-            // kTileN/64 boxes of {64 n (contiguous), kTileK k}: 8 KB each, 128B-swizzled by the k row; with CL = 2
-            // this CTA fetches its half of the boxes and multicasts them
+            // pieces of {64 n (contiguous), kRowsK k}, 128B-swizzled by the k row; block j of 64 n at j * 8 KB
+            using P = BmnPieces<CL>;
 #pragma unroll
-            for (int j = 0; j < kTileN / 64 / CL; ++j) {
-              const int jj = crank * (kTileN / 64 / CL) + j;
-              uint8_t* dst = a_dst + kABytes + jj * (kTileK * 128);
-              if (CL > 1) tma_load_2d_mc(dst, &tmap_b, &full_bar[stage], n0 + jj * 64, kb * kTileK, kAllCtas);
-              else tma_load_2d(dst, &tmap_b, &full_bar[stage], n0 + jj * 64, kb * kTileK);
+            for (int j = 0; j < P::kCount / CL; ++j) {
+              const int p = crank * (P::kCount / CL) + j, nb = p / P::kPerBlock, kp = p % P::kPerBlock;
+              uint8_t* dst = a_dst + kABytes + nb * (kTileK * 128) + kp * (P::kRowsK * 128);
+              if (CL > 1) tma_load_2d_mc(dst, &tmap_b, &full_bar[stage], n0 + nb * 64, kb * kTileK + kp * P::kRowsK, kAllCtas);
+              else tma_load_2d(dst, &tmap_b, &full_bar[stage], n0 + nb * 64, kb * kTileK + kp * P::kRowsK);
             }
           } else if (CL > 1) {
             // rows [n0 + crank*kTileN/CL, +kTileN/CL) of B, delivered to every CTA (the map's box has kTileN / CL rows)
@@ -314,108 +281,79 @@ ffn_hw_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ======================================================================= MMA issuer (one lane)
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int ct = cid; ct < num_ct; ct += ncl) {
-        mbar_wait(&acc_empty_bar[acc], acc_phase ^ 1);                 // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * kTileN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);                          // TMA bytes have landed
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * kStageBytes);
-          const uint32_t b_addr = a_addr + kABytes;
-#pragma unroll
-          for (int k = 0; k < kTileK / kUmmaK; ++k) {
-            // K advance: K-major operands move +32 bytes inside the 128-byte swizzle row per UMMA_K of bf16; the
-            // MN-major operand moves two 8-row k groups (2 x 1024 bytes)
-            const uint64_t bdesc = BMN ? make_smem_desc_mn(b_addr + k * (kUmmaK / 8) * 1024) : make_smem_desc(b_addr + k * kUmmaK * 2);
-            umma_f16(tmem_d, make_smem_desc(a_addr + k * kUmmaK * 2), bdesc, BMN ? kInstrDescBMN : kInstrDesc,
-                     (kb | k) != 0 ? 1u : 0u);
-          }
-          // frees the smem slot when these MMAs retire — in every CTA whose multicast load refills it
-          if (CL > 1) umma_commit_mc(&empty_bar[stage], kAllCtas); else umma_commit(&empty_bar[stage]);
-          if (kb == num_kb - 1) umma_commit(&acc_full_bar[acc]);       // accumulator complete -> epilogue
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= kEpilogueWarp0) {
-    // ================================================================== epilogue (8 warps = 2 warpgroups)
-    const int quad = warp & 3;                                         // TMEM lanes 32*quad .. 32*quad+31
-    const int half = (warp - kEpilogueWarp0) >> 2;                     // which 128 of the 256 accumulator columns
-    // Each lane owns one output row and stores 16-byte vectors straight to global memory.  A staged variant (128B-
-    // swizzled shared-memory tile per warp, 4 full 128-byte lines per store instruction) was measured on B200 and was
-    // SLOWER: 29.95 vs 27.25 us for up+GELU (profiles/r2/bert_ops_bench_staged_epilogue.json vs
-    // bert_ops_bench_handwritten_tcgen05.json) — the epilogue is bound by its instruction count (~37 per element with two
-    // outputs and an erf GELU, 2 warps per scheduler), not by store wavefronts, and the staging added instructions.
-    int acc = 0; uint32_t acc_phase = 0;
+  } else {
+    // ============================================================ consumers: 2 warpgroups x 64 rows
+    const int cw = wg - 1;                                             // rows cw*64 .. cw*64+63 of the tile
+    const int wq = warp & 3;                                           // warp within the warpgroup: 16 rows each
+    int stage = 0; uint32_t phase = 0;
     for (int ct = cid; ct < num_ct; ct += ncl) {
       const int m0 = ((ct % tiles_mc) * CL + crank) * kTileM, n0 = (ct / tiles_mc) * kTileN;
-      mbar_wait(&acc_full_bar[acc], acc_phase);
-      tc_fence_after();
-      const int row = m0 + quad * 32 + lane;
-      const size_t row_off = static_cast<size_t>(row) * N;
-#pragma unroll 1
-      for (int c = 0; c < (kTileN / 2) / 32; ++c) {
-        const int col0 = half * (kTileN / 2) + c * 32;
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + acc * kTileN + col0 + (static_cast<uint32_t>(quad * 32) << 16), v);
-        tmem_ld_wait();
-        const int gcol = n0 + col0;
+      float d[64];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {                                  // 8 columns = one 16-byte vector of bf16
-          const int cj = gcol + j * 8;
-          if (cj < N) {                                                // N % 8 == 0: a vector is all-in or all-out
-            if (MODE == MODE_UP) {
-              const uint4 bv = __ldg(reinterpret_cast<const uint4*>(aux + cj));
-              const uint32_t bw[4] = {bv.x, bv.y, bv.z, bv.w};
-              uint32_t zq[4], hq[4];
+      for (int i = 0; i < 64; ++i) d[i] = 0.f;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);                            // TMA bytes have landed
+        const uint32_t a_addr = smem_u32(smem + stage * kStageBytes) + cw * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem + stage * kStageBytes + kABytes);
+        fence_accumulators(d);
+        wgmma_fence();
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float b0 = __uint_as_float(bw[i] << 16), b1 = __uint_as_float(bw[i] & 0xffff0000u);
-                const float z0 = __uint_as_float(v[j * 8 + 2 * i]) + b0, z1 = __uint_as_float(v[j * 8 + 2 * i + 1]) + b1;
-                zq[i] = pack_bf16(z0, z1);
-                hq[i] = pack_bf16(gelu_fast(z0), gelu_fast(z1));
-              }
-              if (row < M) {
-                *reinterpret_cast<uint4*>(out1 + row_off + cj) = make_uint4(zq[0], zq[1], zq[2], zq[3]);
-                *reinterpret_cast<uint4*>(out0 + row_off + cj) = make_uint4(hq[0], hq[1], hq[2], hq[3]);
-              }
-            } else if (row < M) {                                      // (per-lane predicate: no collective below)
-              const uint4 zv = __ldg(reinterpret_cast<const uint4*>(aux + row_off + cj));
-              const uint32_t zw[4] = {zv.x, zv.y, zv.z, zv.w};
-              uint32_t dq[4];
+        for (int k = 0; k < kTileK / kWgmmaK; ++k) {
+          // K advance: K-major operands move +32 bytes inside the 128-byte swizzle row per 16 bf16; the MN-major
+          // operand moves two 8-row k groups (2 x 1024 bytes)
+          const uint64_t adesc = make_smem_desc(a_addr + k * kWgmmaK * 2, 16);
+          if (BMN) wgmma_m64n128k16<1>(d, adesc, make_smem_desc(b_addr + k * (kWgmmaK / 8) * 1024, kTileK * 128));
+          else wgmma_m64n128k16<0>(d, adesc, make_smem_desc(b_addr + k * kWgmmaK * 2, 16));
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        fence_accumulators(d);
+        // this warp's reads of the stage are complete: release it in every CTA whose multicast load refills it
+        if (CL > 1) { if (lane < CL) mbar_arrive_cluster(&empty_bar[stage], lane); }
+        else if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+
+      // epilogue: accumulator d[4i + {0,1}] is (row r, cols 8i + 2(lane%4) + {0,1}), d[4i + {2,3}] is row r + 8
+      const int r0 = m0 + cw * 64 + wq * 16 + (lane >> 2);
+      const int cbase = n0 + 2 * (lane & 3);
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float z0 = __uint_as_float(zw[i] << 16), z1 = __uint_as_float(zw[i] & 0xffff0000u);
-                dq[i] = pack_bf16(__uint_as_float(v[j * 8 + 2 * i]) * dgelu_fast(z0),
-                                  __uint_as_float(v[j * 8 + 2 * i + 1]) * dgelu_fast(z1));
-              }
-              *reinterpret_cast<uint4*>(out0 + row_off + cj) = make_uint4(dq[0], dq[1], dq[2], dq[3]);
+      for (int i = 0; i < kTileN / 8; ++i) {
+        const int col = cbase + 8 * i;
+        if (col >= N) continue;                                        // N % 8 == 0: a column pair is all-in or all-out
+        if (MODE == MODE_UP) {
+          const uint32_t bw = __ldg(reinterpret_cast<const unsigned int*>(aux + col));
+          const float b0 = __uint_as_float(bw << 16), b1 = __uint_as_float(bw & 0xffff0000u);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = r0 + 8 * h;
+            if (row < M) {
+              const float z0 = d[4 * i + 2 * h] + b0, z1 = d[4 * i + 2 * h + 1] + b1;
+              const size_t off = static_cast<size_t>(row) * N + col;
+              *reinterpret_cast<uint32_t*>(out1 + off) = pack_bf16(z0, z1);
+              *reinterpret_cast<uint32_t*>(out0 + off) = pack_bf16(gelu_fast(z0), gelu_fast(z1));
+            }
+          }
+        } else {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = r0 + 8 * h;
+            if (row < M) {
+              const size_t off = static_cast<size_t>(row) * N + col;
+              const uint32_t zw = __ldg(reinterpret_cast<const unsigned int*>(aux + off));
+              const float z0 = __uint_as_float(zw << 16), z1 = __uint_as_float(zw & 0xffff0000u);
+              *reinterpret_cast<uint32_t*>(out0 + off) =
+                  pack_bf16(d[4 * i + 2 * h] * dgelu_fast(z0), d[4 * i + 2 * h + 1] * dgelu_fast(z1));
             }
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty_bar[acc]);                 // 8 arrivals free the accumulator stage
-      if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
     }
   }
 
   // ------------------------------------------------------------------------------------- teardown
-  tc_fence_before();
   __syncthreads();
   if (CL > 1) cluster_sync_all();                        // no multicast / remote arrive may target a CTA that has exited
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 // -------------------------------------------------------------------------------------------- host
@@ -434,31 +372,17 @@ static EncodeTiledFn encode_tiled() {
   return fn;
 }
 
-// 2-D row-major bf16 matrix [rows, cols]; box = box_rows x 64 columns (128 bytes = one swizzle row)
-static CUtensorMap make_tmap(const void* base, int64_t rows, int64_t cols, int box_rows) {
+// 2-D row-major bf16 matrix [rows, cols]; box = box_rows x box_cols (box_cols = 64: 128 bytes = one swizzle row)
+static CUtensorMap make_tmap(const void* base, int64_t rows, int64_t cols, int box_rows, int box_cols) {
   CUtensorMap m;
   const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
   const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(cols) * 2};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(kTileK), static_cast<cuuint32_t>(box_rows)};
+  const cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
   const cuuint32_t estr[2] = {1, 1};
   CUresult r = encode_tiled()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   TORCH_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with code ", static_cast<int>(r));
-  return m;
-}
-
-// Row-major bf16 matrix [rows = K, cols = N] read as an MN-major operand: box = 64 columns (128 bytes) x kTileK rows
-static CUtensorMap make_tmap_mn(const void* base, int64_t rows, int64_t cols) {
-  CUtensorMap m;
-  const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
-  const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(cols) * 2};
-  const cuuint32_t box[2] = {64u, static_cast<cuuint32_t>(kTileK)};
-  const cuuint32_t estr[2] = {1, 1};
-  CUresult r = encode_tiled()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  TORCH_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (MN-major) failed with code ", static_cast<int>(r));
   return m;
 }
 
@@ -472,8 +396,10 @@ static void check_bf16(const at::Tensor& t, const char* what) {
 template <int MODE, bool BMN, int CL>
 static void launch_hw_cl(const at::Tensor& a, const at::Tensor& b, const __nv_bfloat16* aux, at::Tensor& out0, at::Tensor* out1,
                          int M, int N, int K) {
-  const CUtensorMap ta = hw::make_tmap(a.data_ptr(), M, K, hw::kTileM);
-  const CUtensorMap tb = BMN ? hw::make_tmap_mn(b.data_ptr(), K, N) : hw::make_tmap(b.data_ptr(), N, K, hw::kTileN / CL);
+  const CUtensorMap ta = hw::make_tmap(a.data_ptr(), M, K, hw::kTileM, hw::kTileK);
+  // MN-major B: row-major [K, N] read in pieces of 64 columns (128 bytes) x kRowsK rows
+  const CUtensorMap tb = BMN ? hw::make_tmap(b.data_ptr(), K, N, hw::BmnPieces<CL>::kRowsK, 64)
+                             : hw::make_tmap(b.data_ptr(), N, K, hw::kTileN / CL, hw::kTileK);
   static std::once_flag attr_once;
   std::call_once(attr_once, [] {
     C10_CUDA_CHECK(cudaFuncSetAttribute(hw::ffn_hw_kernel<MODE, BMN, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, hw::kSmemBytes));
@@ -520,8 +446,6 @@ static void launch_hw(const at::Tensor& a, const at::Tensor& b, const __nv_bfloa
                       int M, int N, int K) {
   const int tiles_m = (M + hw::kTileM - 1) / hw::kTileM;
   // the CTAs of a cluster take vertically adjacent tiles: the cluster size must divide the number of tile rows
-  // default 1: measured on B200 the epilogue, not the operand traffic, bounds the kernel, and clusters of 2 / 4 are within
-  // noise of / slightly behind single CTAs (27.6 / 27.8 / 28.4 us, profiles/r2/bert_ops_bench_r2_final.json)
   int cl = g_force_cluster > 0 ? g_force_cluster : 1;
   while (cl > 1 && tiles_m % cl != 0) cl >>= 1;
   if (cl >= 4) launch_hw_cl<MODE, BMN, 4>(a, b, aux, out0, out1, M, N, K);
@@ -529,7 +453,7 @@ static void launch_hw(const at::Tensor& a, const at::Tensor& b, const __nv_bfloa
   else launch_hw_cl<MODE, BMN, 1>(a, b, aux, out0, out1, M, N, K);
 }
 
-// H, Z = gelu(X W^T + b), X W^T + b      (experimental: see the header of this file)
+// H, Z = gelu(X W^T + b), X W^T + b
 std::vector<at::Tensor> ffn_up_hw(const at::Tensor& x, const at::Tensor& w, const at::Tensor& bias) {
   check_bf16(x, "ffn_up_hw x"); check_bf16(w, "ffn_up_hw w"); check_bf16(bias, "ffn_up_hw bias");
   TORCH_CHECK(x.dim() == 2 && w.dim() == 2 && x.size(1) == w.size(1) && bias.numel() == w.size(0), "ffn_up_hw: shape mismatch");
@@ -544,7 +468,7 @@ std::vector<at::Tensor> ffn_up_hw(const at::Tensor& x, const at::Tensor& w, cons
 }
 
 // dZ = (dY Wt^T) * gelu'(Z)   with   Wt = W^T stored [N, K] row-major (K-major operand: the caller keeps a transposed
-// copy of the down-projection weight W [K, N]; an MN-major operand path is the next step, tools/checks/README.md)
+// copy of the down-projection weight W [K, N])
 at::Tensor ffn_dgelu_hw(const at::Tensor& dy, const at::Tensor& wt, const at::Tensor& z) {
   check_bf16(dy, "ffn_dgelu_hw dy"); check_bf16(wt, "ffn_dgelu_hw wt"); check_bf16(z, "ffn_dgelu_hw z");
   TORCH_CHECK(dy.dim() == 2 && wt.dim() == 2 && z.dim() == 2 && dy.size(1) == wt.size(1) && z.size(0) == dy.size(0) &&

@@ -4,7 +4,7 @@ The reference benchmarks HuggingFace ``BertForPreTraining`` built from ``bert_co
 ``bert_base_config.json`` with the vocabulary padded to a multiple of 8 (30522 -> 30528)
 (dear/bert_benchmark.py:72-83).  This is an independent implementation of the same architecture
 (same parameter tensors and tying: the MLM decoder shares the word-embedding matrix), written for
-Blackwell: attention goes through ``scaled_dot_product_attention`` (flash kernels) and the QKV
+Hopper: attention goes through ``scaled_dot_product_attention`` (flash kernels) and the QKV
 projections are one fused GEMM.
 """
 from __future__ import annotations
@@ -122,8 +122,8 @@ class BertSelfAttention(nn.Module):
         p = self.p_drop if self.training else 0.0
         backend = self.backend
         if backend is None and x.is_cuda and S <= 128 and attn_bias is not None and _EFFICIENT is not None:
-            # short sequences with a key-padding bias: the memory-efficient kernel beats cuDNN's 128x128-tile flash
-            # backward (55 vs 77 us forward+backward at batch 32 x 16 heads x 64 x 64, profiles/bert_ops_bench.json)
+            # short sequences with a key-padding bias: the memory-efficient kernel instead of cuDNN's 128x128-tile
+            # flash backward (tools/bert_ops_bench.py --ops attn compares them)
             backend = _EFFICIENT
         if backend is None:
             o = F.scaled_dot_product_attention(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), attn_mask=attn_bias,
@@ -138,7 +138,7 @@ class BertSelfAttention(nn.Module):
 class BertLayer(nn.Module):
     """Post-LN transformer layer.  ``fused_ln``: bias + dropout + add + LayerNorm in one kernel
     (ops/fused_ln.py) and bias + GELU in one kernel (ops/bias_gelu.py), bias gradients fused into their
-    backward kernels; ``tc_ffn``: feed-forward block on the tcgen05 GEMMs with GELU / GELU' in the
+    backward kernels; ``tc_ffn``: feed-forward block on the wgmma GEMMs with GELU / GELU' in the
     epilogues (ops/tc_gemm.py).  Parameters and state-dict keys are identical in every mode."""
 
     def __init__(self, c: BertConfig, fused_ln: bool = False, tc_ffn: bool = False):

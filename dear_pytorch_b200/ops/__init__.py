@@ -2,7 +2,7 @@
 
 The compiled extension ``dear_pytorch_b200._C`` (built in-tree by
 ``python setup.py build_ext --inplace`` or ``__graft_entry__.build()``) holds
-the sm_100a kernels and the C++ runtime.  On a machine with a GPU the
+the sm_90a kernels and the C++ runtime.  On a machine with a GPU the
 extension is mandatory: there is no silent PyTorch fallback for the fused
 path (``require_native`` raises).  On CPU-only machines the same extension
 provides the host-emulation backend.

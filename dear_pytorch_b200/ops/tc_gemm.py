@@ -1,4 +1,4 @@
-"""Transformer feed-forward block on the hand-written tcgen05 GEMMs of ``csrc/tc_ffn_hw.cu`` (opt-in: ``--tc-ffn 1``).
+"""Transformer feed-forward block on the hand-written wgmma GEMMs of ``csrc/tc_ffn_hw.cu`` (opt-in: ``--tc-ffn 1``).
 
 ``fused_ffn(x, w1, b1, w2, b2)`` = ``linear(gelu(linear(x, w1, b1)), w2, b2)`` with
 
@@ -39,7 +39,7 @@ def tc_native():
 def require_tc():
     mod = tc_native()
     if mod is None:
-        raise RuntimeError("dear_pytorch_b200._tc (tcgen05 GEMMs) is not built: %r -- run "
+        raise RuntimeError("dear_pytorch_b200._tc (wgmma GEMMs) is not built: %r -- run "
                            "`python setup.py build_ext --inplace`" % (_tc_error,))
     return mod
 
@@ -87,7 +87,7 @@ class _FusedFFN(torch.autograd.Function):
 
 
 def fused_ffn(x, w1, b1, w2, b2):
-    """``linear(gelu(linear(x, w1, b1)), w2, b2)``; tcgen05 kernels on CUDA bf16."""
+    """``linear(gelu(linear(x, w1, b1)), w2, b2)``; wgmma kernels on CUDA bf16."""
     if _eligible(x, w1, w2):
         return _FusedFFN.apply(x, w1, b1, w2, b2)
     return F.linear(F.gelu(F.linear(x, w1, b1)), w2, b2)

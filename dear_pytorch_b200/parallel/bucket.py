@@ -13,7 +13,7 @@ Reference rules (SURVEY.md §8.2-8.3):
   * flags          dear/dopt_rsag_wt.py:216-241 a boundary flag per module.
   * per tensor     dear/dopt_rsag_naive.py     one bucket per module ("w/o tensor fusion").
 
-Layout differences (deliberate, B200-first):
+Layout differences (deliberate, GPU-first):
   * every parameter starts on a 256-byte boundary inside its bucket so that the views handed
     to cuDNN/cuBLAS (and TMA-based kernels) are aligned and so that hyper-parameter segments
     never straddle a 128-bit vector;

@@ -6,7 +6,7 @@ bucket while the backward pass is still running, and the matching all-gather plu
 SGD update are overlapped with the forward pass of iteration *t+1*.  The result is
 mathematically identical to synchronous data-parallel SGD.
 
-B200-first redesign (SURVEY.md §7, §9):
+GPU-first redesign (SURVEY.md §7, §9):
   * parameters live in flat symmetric *parameter buckets* (``p.data`` is a view) and the
     update is **sharded**: each rank updates 1/P of every bucket (momentum and fp32 master
     state are sharded too) and pushes the result into every peer's bucket — Kernel B;

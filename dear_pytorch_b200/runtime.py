@@ -9,7 +9,7 @@ Here:
     no MPI.  A process started without those variables is a world of one.
   * the device is pinned from LOCAL_RANK (not a hard-coded ``% 4``).
   * ``backend`` selects the data path of the decoupled all-reduce:
-      "b200"  our fused sm_100a kernels over peer-mapped NVLink memory  (default on GPU)
+      "b200"  our fused sm_90a kernels over peer-mapped NVLink memory  (default on GPU)
       "emu"   the same native runtime executed on the host over POSIX shm (CPU tests)
       "nccl"  torch.distributed NCCL collectives + eager update          (baseline)
       "gloo"  torch.distributed gloo collectives + eager update          (CPU plumbing)
@@ -135,8 +135,7 @@ def init(backend: Optional[str] = None, device: Optional[torch.device] = None, *
         # CTAs of the fused kernels (upper bounds; small buckets get fewer, csrc/communicator.cpp: grid_for).  On one GPU
         # nothing ever spins, so the kernels may take most of the chip for a few microseconds (HBM-bound).  With peers
         # the pull is NVLink-bound from ~32 CTAs on, but the PACK phase of Kernel A and the push of Kernel B scale with
-        # the CTA count (2 B200s, 392 MB bucket, profiles/r2/kernelA_oneshot_grid_sweep_p2.log: Kernel A 615 / 525 /
-        # 490 / 460 us and Kernel B 508 / 358 / 386 / 343 us at 32 / 48 / 64 / 96 CTAs; NCCL 500 / 495 us).
+        # the CTA count (tools/kernel_bench.py sweeps it).
         o.rs_grid = _env_int("DEAR_RS_GRID", 128 if world == 1 else 64)
         o.ag_grid = _env_int("DEAR_AG_GRID", 128 if world == 1 else 48)
         o.gen_grid = _env_int("DEAR_GEN_GRID", 8)

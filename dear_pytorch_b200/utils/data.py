@@ -15,8 +15,7 @@ Contract: a batch returned by ``next()`` stays valid until the work enqueued bef
 ``upload_delay_us``: a ring slot frees when the previous step's work retires, so every upload starts exactly at a
 step boundary.  With the rotated training step (``TrainStep(overlap_update=True)``) the first thing a step runs is
 Kernel B — the sharded update + all-gather, whose flag traffic uses system-scope release/acquire — and the PCIe DMA
-landing at the same moment measurably stretches it (end-to-end minus device-resident step time: 0.01 ms with the
-natural body, 0.18 ms with the rotated one at 1 GPU; profiles/bench_default_1gpu*.json).  A short spin on the COPY
+landing at the same moment can stretch it (compare bench.py's end-to-end and device-resident step times).  A short spin on the COPY
 stream in front of each upload moves the DMA into the forward pass, where the natural body already shows it is
 free.  The copy still completes one and a half steps before its batch is consumed.
 """

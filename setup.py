@@ -1,7 +1,7 @@
 """Build the native runtime in-tree:  python setup.py build_ext --inplace
 
 Produces dear_pytorch_b200/_C.*.so (runtime, collectives, fused BN / LN kernels) and dear_pytorch_b200/_tc.*.so
-(hand-written tcgen05 GEMMs with fused epilogues) -- sm_100a only; no other architecture is built.
+(hand-written wgmma / TMA GEMMs with fused epilogues) -- sm_90a (H100) only; no other architecture is built.
 The reference's counterpart is common/comm_core/setup.py:16-44 (NCCL+MPI); this
 extension links neither.
 """
@@ -15,7 +15,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join("dear_pytorch_b200", "csrc")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xptxas", "-v",
     "--expt-relaxed-constexpr",
@@ -35,7 +35,7 @@ ext = CUDAExtension(
 
 tc_ext = CUDAExtension(
     name="dear_pytorch_b200._tc",
-    # hand-written tcgen05 / TMEM / TMA kernels (raw PTX; no CUTLASS headers needed)
+    # hand-written wgmma / TMA kernels (raw PTX; no CUTLASS headers needed)
     sources=[os.path.join(CSRC, "tc_bindings.cpp"), os.path.join(CSRC, "tc_ffn_hw.cu")],
     include_dirs=[os.path.join(ROOT, CSRC)],
     extra_compile_args={"cxx": CXX_FLAGS, "nvcc": NVCC_FLAGS},

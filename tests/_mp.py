@@ -4,6 +4,7 @@ import socket
 import sys
 import traceback
 
+import cloudpickle
 import torch
 import torch.multiprocessing as mp
 
@@ -26,6 +27,8 @@ def _worker(rank, world, port, backend, fn, args, ret, extra_env):
         sys.path.insert(0, ROOT)
     torch.set_num_threads(1)
     try:
+        if isinstance(fn, bytes):
+            fn = cloudpickle.loads(fn)
         import dear_pytorch_b200 as dear
         dear.init()
         out = fn(rank, world, *args)
@@ -39,12 +42,21 @@ def _worker(rank, world, port, backend, fn, args, ret, extra_env):
 def run_ranks(fn, world=2, backend="gloo", args=(), timeout=240, extra_env=None, start_method=None):
     """Run ``fn(rank, world, *args)`` on ``world`` processes; returns the list of results.
 
-    CPU backends fork (the children inherit the already-imported torch: ~10x faster than spawn);
-    anything touching CUDA must spawn.
+    CPU backends fork (the children inherit the already-imported torch: ~10x faster than spawn) on a machine without a
+    GPU.  Where a GPU is visible, autograd keeps worker threads per device once this process has run a backward pass,
+    and a child forked after that cannot run one: there the children of a CPU backend come from a fork server that has
+    imported torch and nothing else.  Anything touching CUDA must spawn.
     """
     if start_method is None:
-        start_method = "fork" if backend in ("gloo", "emu") and not torch.cuda.is_initialized() else "spawn"
+        if backend in ("gloo", "emu") and not torch.cuda.is_initialized():
+            start_method = "fork" if torch.cuda.device_count() == 0 else "forkserver"
+        else:
+            start_method = "spawn"
     ctx = mp.get_context(start_method)
+    if start_method == "forkserver":
+        ctx.set_forkserver_preload(["torch"])
+    if start_method != "fork":
+        fn = cloudpickle.dumps(fn)          # by value when it is not importable (a worker defined inside a test)
     mgr = ctx.Manager()
     ret = mgr.dict()
     port = free_port()

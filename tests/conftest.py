@@ -12,7 +12,7 @@ os.environ.setdefault("PYTHONPATH", ROOT + os.pathsep + os.environ.get("PYTHONPA
 def pytest_configure(config):
     import torch
     torch.set_num_threads(1)      # no OpenMP pool in the parent: children are forked
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (pytest -m gpu on an H100)")
     config.addinivalue_line("markers", "multigpu: needs >= 2 CUDA devices")
 
 

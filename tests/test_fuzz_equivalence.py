@@ -2,12 +2,14 @@
 re-bucketing / state-dict round trips on 2-4 ranks against single-process torch.optim."""
 import importlib.util
 import os
+import sys
 
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 spec = importlib.util.spec_from_file_location("fuzz_equivalence", os.path.join(ROOT, "tools", "fuzz_equivalence.py"))
 fuzz = importlib.util.module_from_spec(spec)
+sys.modules["fuzz_equivalence"] = fuzz      # rank processes that do not fork find `worker` under this name
 spec.loader.exec_module(fuzz)
 
 

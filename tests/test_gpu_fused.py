@@ -1,4 +1,4 @@
-"""GPU tests of the fused path (run on the B200 box: pytest -m gpu).
+"""GPU tests of the fused path (pytest -m gpu on an H100).
 
 Numerics oracle: plain PyTorch fp32 SGD on the concatenated batch.  Multi-rank cases run one
 process per rank; with a single GPU all ranks share cuda:0 (CUDA IPC works between processes on one

@@ -1,4 +1,4 @@
-"""Hand-written tcgen05 GEMMs with fused epilogues (csrc/tc_ffn_hw.cu) against plain PyTorch fp32 references."""
+"""Hand-written wgmma GEMMs with fused epilogues (csrc/tc_ffn_hw.cu) against plain PyTorch fp32 references."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -66,7 +66,7 @@ def test_handwritten_ffn_dgelu(M, K, N):
 @pytest.mark.parametrize("M,K,N", [(128, 64, 256), (2048, 1024, 4096), (300, 72, 264), (5, 8, 16)])
 def test_handwritten_ffn_dgelu_mn_major_weight(M, K, N):
     """Same op with the weight [K, N] as nn.Linear stores it: the B operand is MN-major (TMA boxes of 64 contiguous n,
-    UMMA descriptor with LBO/SBO of the MN-major canonical layout) — no transposed copy."""
+    wgmma descriptor with LBO/SBO of the MN-major canonical layout, transposed B) — no transposed copy."""
     tc = require_tc()
     dev = torch.device("cuda:0")
     torch.manual_seed(2)
@@ -83,7 +83,7 @@ def test_handwritten_ffn_dgelu_mn_major_weight(M, K, N):
 @pytest.mark.parametrize("M,K,N", [(2048, 1024, 4096), (512, 192, 512), (1024, 64, 264)])
 def test_handwritten_kernels_with_multicast_clusters(M, K, N, cl):
     """CL CTAs per cluster share the B tile: each loads 1/CL of it and multicasts (cp.async.bulk.tensor ...
-    .multicast::cluster), the MMA warp releases a stage in every CTA (tcgen05.commit ... multicast::cluster)."""
+    .multicast::cluster), every consumer warp releases a stage in every CTA (remote mbarrier arrive)."""
     tc = require_tc()
     dev = torch.device("cuda:0")
     torch.manual_seed(4)

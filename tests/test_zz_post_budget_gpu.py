@@ -1,4 +1,4 @@
-"""GPU runs of everything that was written AFTER the round's GPU budget was spent (profiles/README.md R2.0).
+"""GPU runs of the features written last: gradient clipping, optimizer branches, autocast, rotated graphs, fuzz slice.
 
 These features were developed against the CPU backends only — same Python engine, same C++ runtime, kernels emulated on
 the host — and have never executed on hardware by the time they were committed.  The file sorts last on purpose: whatever

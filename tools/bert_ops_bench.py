@@ -58,16 +58,16 @@ def _graph_time(fn, iters):
 
 
 def _gemm_section(r, tc, x, w1, b1, w2, b2, h, z, dy):
-    """The FFN's two fusable GEMMs: library path (cuBLAS + elementwise kernels) vs the hand-written tcgen05 kernels
+    """The FFN's two fusable GEMMs: library path (cuBLAS + elementwise kernels) vs the hand-written wgmma kernels
     (csrc/tc_ffn_hw.cu) with 1 / 2 / 4 CTAs per cluster sharing the B tile through TMA multicast."""
     # 1. up projection + bias + GELU (forward)
     r["up_gelu_eager"] = graph_time(lambda: F.gelu(F.linear(x, w1, b1)))
     r["up_gemm_only_cublas"] = graph_time(lambda: F.linear(x, w1, b1))
     for cl in (1, 2, 4):
         tc.set_ffn_hw_cluster(cl)
-        r["up_gelu_tcgen05_handwritten_cl%d" % cl] = graph_time(lambda: tc.ffn_up_hw(x, w1, b1))
+        r["up_gelu_wgmma_handwritten_cl%d" % cl] = graph_time(lambda: tc.ffn_up_hw(x, w1, b1))
     tc.set_ffn_hw_cluster(-1)
-    r["up_gelu_tcgen05_handwritten"] = graph_time(lambda: tc.ffn_up_hw(x, w1, b1))
+    r["up_gelu_wgmma_handwritten"] = graph_time(lambda: tc.ffn_up_hw(x, w1, b1))
     # 2. down projection (forward): plain GEMM, cuBLAS in both paths
     r["down_eager"] = graph_time(lambda: F.linear(h, w2, b2))
     # 3. dgrad of the down projection + GELU backward
@@ -78,11 +78,11 @@ def _gemm_section(r, tc, x, w1, b1, w2, b2, h, z, dy):
     r["dgrad_gemm_only_cublas"] = graph_time(lambda: dy.mm(w2))
     for cl in (1, 2, 4):
         tc.set_ffn_hw_cluster(cl)
-        r["dgrad_dgelu_tcgen05_handwritten_cl%d" % cl] = graph_time(lambda: tc.ffn_dgelu_hw_nt(dy, w2, z))
+        r["dgrad_dgelu_wgmma_handwritten_cl%d" % cl] = graph_time(lambda: tc.ffn_dgelu_hw_nt(dy, w2, z))
     tc.set_ffn_hw_cluster(-1)
-    r["dgrad_dgelu_tcgen05_handwritten"] = graph_time(lambda: tc.ffn_dgelu_hw_nt(dy, w2, z))
+    r["dgrad_dgelu_wgmma_handwritten"] = graph_time(lambda: tc.ffn_dgelu_hw_nt(dy, w2, z))
     w2t = w2.t().contiguous()
-    r["dgrad_dgelu_tcgen05_handwritten_kmajor_needs_transpose"] = graph_time(lambda: tc.ffn_dgelu_hw(dy, w2t, z))
+    r["dgrad_dgelu_wgmma_handwritten_kmajor_needs_transpose"] = graph_time(lambda: tc.ffn_dgelu_hw(dy, w2t, z))
 
 
 def main():
@@ -92,7 +92,7 @@ def main():
     ap.add_argument("--inter", type=int, default=4096)
     ap.add_argument("--json", default=None)
     ap.add_argument("--sections", default="gemm,ffn,ln,lg,attn",
-                    help="comma list: gemm (tcgen05 variants vs cuBLAS), ffn (whole block), ln, lg (linear+gelu), attn")
+                    help="comma list: gemm (wgmma variants vs cuBLAS), ffn (whole block), ln, lg (linear+gelu), attn")
     a = ap.parse_args()
     sections = set(a.sections.split(","))
     dev = torch.device("cuda:0")
@@ -129,7 +129,7 @@ def main():
         return torch.autograd.grad(y, [xs] + ps, dy)
     if "ffn" in sections:
         r["ffn_fwd_bwd_eager"] = graph_time(ffn_eager)
-        r["ffn_fwd_bwd_tcgen05_handwritten"] = graph_time(ffn_fused)
+        r["ffn_fwd_bwd_wgmma_handwritten"] = graph_time(ffn_fused)
 
     # 5. dropout + add + LayerNorm, forward + backward
     av = x.clone().requires_grad_(True)
@@ -208,9 +208,9 @@ def main():
     for k in list(r):
         r[k] = round(r[k], 2)
     if "gemm" in sections:
-        out["tflops"] = {"up_gelu_tcgen05_handwritten": round(flops_up / r["up_gelu_tcgen05_handwritten"] / 1e6, 1),
+        out["tflops"] = {"up_gelu_wgmma_handwritten": round(flops_up / r["up_gelu_wgmma_handwritten"] / 1e6, 1),
                          "up_gemm_only_cublas": round(flops_up / r["up_gemm_only_cublas"] / 1e6, 1),
-                         "dgrad_dgelu_tcgen05_handwritten": round(flops_up / r["dgrad_dgelu_tcgen05_handwritten"] / 1e6, 1),
+                         "dgrad_dgelu_wgmma_handwritten": round(flops_up / r["dgrad_dgelu_wgmma_handwritten"] / 1e6, 1),
                          "dgrad_gemm_only_cublas": round(flops_up / r["dgrad_gemm_only_cublas"] / 1e6, 1)}
     print(json.dumps(out, indent=1))
     if a.json:

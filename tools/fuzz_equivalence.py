@@ -23,6 +23,8 @@ import torch.nn as nn
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+# rank processes that do not fork (spawn / fork server) import this module by name to find `worker`
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 from _mp import run_ranks  # noqa: E402
 
 

@@ -8,8 +8,8 @@ For every bucket size it times (CUDA events, after warm-up, max over ranks)
   Kernel B  ag_kernel : sharded SGD(momentum) + all-gather push
 and the NCCL collectives the reference issues for the same bucket
 (reduce_scatter_tensor / all_gather_into_tensor, without the reference's extra elementwise kernels).
-Bus bandwidth = bytes * (P-1)/P / time, reported against the measured 770 GB/s per direction
-(nominal 900 GB/s) from B200_PROFILING.md; at P = 1 the HBM roofline applies instead.
+Bus bandwidth = bytes * (P-1)/P / time, reported against the H100 SXM data sheet's 450 GB/s per direction
+(utils/perf_model.py); at P = 1 the HBM roofline applies instead.
 """
 import argparse
 import json

@@ -4,7 +4,7 @@
     ncu --set full --clock-control none --import-source on -k regex:'ffn_hw_kernel|ln_fwd_kernel|ln_bwd_kernel|bias_gelu_bwd' \
         --launch-skip 10 --launch-count 5 -o gpurun_out/prof_bert_ops python tools/ncu_bert_ops.py
 
-Per iteration, in order: hand-written tcgen05 GEMM+bias+GELU, dgrad GEMM x GELU' (MN-major weight), fused dropout+add+LN
+Per iteration, in order: hand-written wgmma GEMM+bias+GELU, dgrad GEMM x GELU' (MN-major weight), fused dropout+add+LN
 forward, its backward, bias+GELU backward (5 kernels matching the regex above)."""
 import os
 import sys

@@ -1,4 +1,4 @@
-// p2p_probe.cu — what can one B200 pull from / push to its NVSwitch peers, and with which instruction?
+// p2p_probe.cu — what can one H100 pull from / push to its NVSwitch peers, and with which instruction?
 //
 // Single process, N devices with peer access enabled.  Every device d runs the SAME access pattern the
 // fused reduce-scatter / all-gather kernels use (csrc/kernels.cu):
@@ -10,7 +10,7 @@
 //         tma    : cp.async.bulk global->shared (UBLKCP) ring with mbarriers, reduce from shared memory
 //   push  stg_na : st.global.L1::no_allocate.v4
 //         tma    : cp.async.bulk shared->global (UBLKCP) to every peer
-// Build:  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o build/p2p_probe tools/p2p_probe.cu
+// Build:  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o build/p2p_probe tools/p2p_probe.cu
 // Run  :  build/p2p_probe [ndev] [bucket_mb] [grids e.g. 16,32,64,128]
 #include <cuda_runtime.h>
 #include <cstdint>

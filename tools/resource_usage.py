@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Registers / shared memory / spills per kernel family of the built extensions (cuobjdump --dump-resource-usage; no GPU
-needed).  `python tools/resource_usage.py > profiles/r2/resource_usage.txt`"""
+needed).  `python tools/resource_usage.py`"""
 import collections
 import glob
 import os
@@ -41,7 +41,7 @@ def main():
             f["stack"] = max(f["stack"], stack)
             f["local"] = max(f["local"], local)
             f["shared"].add(shared)
-        print("== %s (sm_100a)" % os.path.basename(so))
+        print("== %s (sm_90a)" % os.path.basename(so))
         print("%-34s %5s %9s %14s %6s %6s" % ("kernel family", "inst.", "regs", "static smem B", "stack", "local"))
         for fam, f in fams.items():
             regs = "%d" % f["reg"][0] if min(f["reg"]) == max(f["reg"]) else "%d-%d" % (min(f["reg"]), max(f["reg"]))

@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """Instruction-mix evidence for the hand-written kernels: which SASS the peer / TMA / tensor-core paths compile to.
 
-    python tools/sass_summary.py > profiles/r2/sass_summary_r2.txt
+    python tools/sass_summary.py
 
-Reads the in-tree extensions with ``cuobjdump -sass`` (works without a GPU).  Mnemonics that prove the Blackwell paths
-(B200_PROFILING.md): ``UTCHMMA`` = tcgen05.mma, ``LDTM`` = tcgen05.ld, ``UTMALDG`` = cp.async.bulk.tensor, ``UBLKCP`` =
-cp.async.bulk, ``SYNCS`` = mbarrier, ``LDGMC`` / ``REDG``-style multimem = NVLS.
+Reads the in-tree extensions with ``cuobjdump -sass`` (works without a GPU).  Mnemonics that prove the Hopper paths:
+``HGMMA`` = wgmma.mma_async, ``UTMALDG`` = cp.async.bulk.tensor, ``UBLKCP`` = cp.async.bulk, ``SYNCS`` = mbarrier,
+``LDGMC`` / ``REDG``-style multimem = NVLS.
 """
 import collections
 import glob
@@ -13,8 +13,8 @@ import re
 import subprocess
 import sys
 
-WANT = re.compile(r"^(UTC\w+|LDTM|STTM|UTMALDG|UTMASTG|UBLKCP|SYNCS|LDGMC|LDG|STG|ATOMG|REDG|RED|MEMBAR|FENCE|ERRBAR|BAR|"
-                  r"LDS|STS|NANOSLEEP|ELECT|UTCBAR|UTCATOMSWS|R2UR|CCTL)")
+WANT = re.compile(r"^(HGMMA|WARPGROUP|UTMALDG|UTMASTG|UBLKCP|SYNCS|LDGMC|LDG|STG|ATOMG|REDG|RED|MEMBAR|FENCE|ERRBAR|BAR|"
+                  r"LDS|STS|NANOSLEEP|ELECT|R2UR|CCTL)")
 KERNELS = ["rs_kernelIfLi8ELb0", "rs_kernelIfLi8ELb1", "rs_kernelI13__nv_bfloat16Li8ELb0", "rs_pipe_kernelIf",
            "rs_pipe_kernelI13__nv_bfloat16", "ag_kernelIfLi8ELb0ELb0", "ag_kernelIfLi8ELb1ELb0", "ffn_hw_kernelILi0ELb0",
            "ffn_hw_kernelILi1ELb0", "ffn_hw_kernelILi1ELb1"]
