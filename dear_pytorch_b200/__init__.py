@@ -15,6 +15,7 @@ checkpointing (``save_checkpoint`` / ``load_checkpoint``) and a CUDA-graph step 
 from .runtime import (init, shutdown, rank, size, local_rank, local_size, backend, device, barrier,  # noqa: F401
                       is_initialized, communicator)
 from .parallel.optimizer import DistributedOptimizer, DearEngine, THRESHOLD, NUM_NEARBY_LAYERS  # noqa: F401
+from .parallel.grad_scaler import GradScaler  # noqa: F401
 from .parallel.collectives import (allreduce, allreduce_, broadcast_, broadcast_parameters,  # noqa: F401
                                    broadcast_optimizer_state, allgather)
 from .utils.checkpoint import save_checkpoint, load_checkpoint  # noqa: F401

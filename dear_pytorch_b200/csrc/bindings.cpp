@@ -119,7 +119,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("set_grad_scale", &BucketSet::set_grad_scale, py::arg("scale"))
       .def("pack_pieces", &BucketSet::pack_pieces, py::arg("bucket"))
       .def("allgather_update", &BucketSet::allgather_update, py::arg("bucket"), py::arg("do_update") = true,
-           py::arg("first_step") = false, py::arg("entry_barrier") = true, py::arg("zero_grad") = false)
+           py::arg("first_step") = false, py::arg("entry_barrier") = true, py::arg("zero_grad") = false,
+           py::arg("amp_decide") = false)
+      .def("set_amp", &BucketSet::set_amp, py::arg("state"))
+      .def("join", &BucketSet::join, py::arg("other"))
       .def("fence_current_to_comm", &BucketSet::fence_current_to_comm)
       .def("wait_bucket", &BucketSet::wait_bucket)
       .def("wait_rs", &BucketSet::wait_rs)

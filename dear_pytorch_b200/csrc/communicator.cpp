@@ -431,6 +431,7 @@ BucketSet::BucketSet(std::shared_ptr<Communicator> comm, std::vector<int64_t> pa
     ag_stream_ = o.separate_ag_stream ? make_priority_stream() : stream_;
     ev_fence_ = make_event();
     ev_fence_ag_ = make_event();
+    ev_join_ = make_event();
     for (auto& b : buckets_) {
       b.ev_in = make_event();
       b.rs_done = make_event();
@@ -459,6 +460,7 @@ BucketSet::~BucketSet() {
     }
     if (ev_fence_) cudaEventDestroy(E(ev_fence_));
     if (ev_fence_ag_) cudaEventDestroy(E(ev_fence_ag_));
+    if (ev_join_) cudaEventDestroy(E(ev_join_));
     if (upload_stream_) cudaStreamDestroy(S(upload_stream_));
     if (ag_stream_ && ag_stream_ != stream_) {
       cudaStreamSynchronize(S(ag_stream_));
@@ -747,6 +749,7 @@ void BucketSet::reduce_scatter(int g, bool pack) {
   p.dtype = dtype_;
   p.status = cuda ? status_word_device() : status_word_host();
   p.timeout_ns = comm_->timeout_ns();
+  p.amp = amp_.defined() ? reinterpret_cast<AmpState*>(amp_.data_ptr()) : nullptr;
   if (b.rs_algo == RS_ALGO_PIPE) {
     // stripe-pipelined variant: stripe-major work list instead of the segment table (device kernel and host emulation)
     p.nstripes = b.nstripes;
@@ -781,7 +784,29 @@ void BucketSet::reduce_scatter(int g, bool pack) {
   comm_->count_launch();
 }
 
-void BucketSet::allgather_update(int g, bool do_update, bool first_step, bool entry_barrier, bool zero_grad) {
+void BucketSet::set_amp(std::optional<torch::Tensor> state) {
+  if (!state.has_value() || !state->defined()) {
+    amp_ = torch::Tensor();
+    return;
+  }
+  const torch::Tensor& t = *state;
+  DEAR_CHECK(t.scalar_type() == torch::kInt && t.is_contiguous() && t.numel() * 4 == static_cast<int64_t>(sizeof(AmpState)),
+             "set_amp: the scaler state must be a contiguous int32 tensor of " << sizeof(AmpState) / 4 << " elements");
+  DEAR_CHECK(t.is_cuda() == comm_->is_cuda() && (!t.is_cuda() || t.device().index() == comm_->options().device),
+             "set_amp: the scaler state lives on the wrong device");
+  amp_ = t;
+}
+
+void BucketSet::join(BucketSet& other) {
+  if (!comm_->is_cuda() || &other == this) return;
+  for (void* st : {other.stream_, other.ag_stream_}) {
+    DEAR_CUDA(cudaEventRecord(E(ev_join_), S(st)));
+    DEAR_CUDA(cudaStreamWaitEvent(S(ag_stream_), E(ev_join_), 0));
+  }
+}
+
+void BucketSet::allgather_update(int g, bool do_update, bool first_step, bool entry_barrier, bool zero_grad,
+                                 bool amp_decide) {
   auto& b = buckets_.at(g);
   const bool cuda = comm_->is_cuda();
   AGParams p;
@@ -811,6 +836,10 @@ void BucketSet::allgather_update(int g, bool do_update, bool first_step, bool en
   p.shard_elems = static_cast<uint64_t>(b.shard);
   p.first_step = first_step ? 1u : 0u;
   p.entry_barrier = entry_barrier ? 1u : 0u;
+  p.amp = amp_.defined() ? reinterpret_cast<AmpState*>(amp_.data_ptr()) : nullptr;
+  DEAR_CHECK(!amp_decide || (p.amp != nullptr && entry_barrier && do_update),
+             "the deciding update of a scaled step needs a scaler state, the entry rendezvous and an update");
+  p.amp_decide = amp_decide ? 1u : 0u;
   p.do_update = do_update ? 1u : 0u;
   p.sig = arena_->sig_table();
   p.ctrl = arena_->ctrl();

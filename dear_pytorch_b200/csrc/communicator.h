@@ -148,7 +148,12 @@ class BucketSet {
   std::string rs_plan(int g) const;
   // the pipelined kernel's work list of bucket g as rows (src, dst_off, nbytes, stripe, flags) — for tests / debugging
   std::vector<std::vector<int64_t>> pack_pieces(int g) const;
-  void allgather_update(int g, bool do_update, bool first_step, bool entry_barrier, bool zero_grad);
+  void allgather_update(int g, bool do_update, bool first_step, bool entry_barrier, bool zero_grad, bool amp_decide = false);
+  // Dynamic loss scaling: `state` is the engine's AmpState (int32[9], on this set's device), or None for the static path.
+  void set_amp(std::optional<torch::Tensor> state);
+  // The next update kernel on this set's all-gather stream waits for everything queued so far on both streams of
+  // `other` (one decision per step across the sets of an engine).
+  void join(BucketSet& other);
   void fence_current_to_comm();
   void wait_bucket(int g);
   void wait_rs(int g);
@@ -210,6 +215,8 @@ class BucketSet {
   void* ev_fence_ag_ = nullptr;
   void* upload_stream_ = nullptr;   // private non-capturing stream for tables built during a capture
   float grad_scale_ = 1.0f;
+  torch::Tensor amp_;               // AmpState of the engine's dynamic loss scaler (undefined: static path)
+  void* ev_join_ = nullptr;
 };
 
 // device launchers (kernels.cu) and host emulation (emu.cpp)

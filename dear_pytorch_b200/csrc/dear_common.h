@@ -156,6 +156,42 @@ DEAR_HD uint32_t find_pack_seg(const PackSeg* segs, uint32_t n, uint32_t t) {
   return lo;
 }
 
+// ---- dynamic loss scaling -----------------------------------------------------
+
+// Device-resident state of a dynamic loss scaler (parallel/grad_scaler.py), one per engine, shared by every BucketSet.
+// Kernel A divides the reduced gradient by `scale` and ORs a non-finite result into `overflow`; the deciding Kernel B of
+// the step agrees on the bit with every rank at its entry rendezvous, writes `found_inf`, applies torch's
+// growth / backoff rule to `scale` and `growth_tracker`, and clears `overflow`.  Nine 32-bit words (torch int32[9]).
+struct AmpState {
+  uint32_t overflow;        // this rank saw a non-finite reduced gradient in the current step
+  uint32_t found_inf;       // decision of the current step (some rank overflowed: skip the update)
+  float scale;
+  int32_t growth_tracker;
+  uint32_t applied;         // updates applied so far (skipped steps excluded)
+  float growth_factor;
+  float backoff_factor;
+  int32_t growth_interval;
+  int32_t prev_growth_tracker;  // growth_tracker before the current step's rule (update(new_scale) restores it)
+};
+
+// torch._amp_update_scale_: back off on overflow, grow after `growth_interval` clean steps in a row.
+DEAR_HD void amp_update_scale(AmpState* a, bool found_inf) {
+  a->prev_growth_tracker = a->growth_tracker;
+  if (found_inf) {
+    a->scale *= a->backoff_factor;
+    a->growth_tracker = 0;
+    return;
+  }
+  const int32_t successful = a->growth_tracker + 1;
+  if (successful == a->growth_interval) {
+    const float grown = a->scale * a->growth_factor;
+    if (grown - grown == 0.f) a->scale = grown;     // finite
+    a->growth_tracker = 0;
+  } else {
+    a->growth_tracker = successful;
+  }
+}
+
 // ---- kernel parameter blocks ------------------------------------------------
 
 // Kernel A: fused [pack local grads -> symmetric bucket] + cross-GPU ready
@@ -187,6 +223,9 @@ struct RSParams {
   // order, stripe k owning entries [piece_first[k], piece_first[k+1])
   const PackSeg* pieces;
   uint32_t piece_first[17];
+  // dynamic loss scale (nullptr => static path): the output is additionally divided by amp->scale, and a non-finite
+  // output value sets amp->overflow
+  AmpState* amp;
 };
 
 // RS_READY flag encoding shared by both reduce-scatter kernels: (epoch << 8) | stripes_published; the one-shot
@@ -218,7 +257,7 @@ struct AGParams {
   uint64_t shard_elems;
   const HyperSeg* hyper;   // device table
   uint32_t nhyper;
-  uint32_t first_step;     // momentum buffers are uninitialised
+  uint32_t first_step;     // momentum buffers are uninitialised (ignored with `amp`: then step_ctr == 0 decides)
   uint32_t entry_barrier;  // wait for every peer to reach this kernel before pushing
   uint32_t do_update;      // 0 => pure all-gather of the shard (no SGD)
   PeerTable sig;
@@ -229,7 +268,15 @@ struct AGParams {
   int dtype;               // DType of the parameter bucket
   uint32_t* status;
   uint64_t timeout_ns;
+  // dynamic loss scale (nullptr => static path): the update is skipped when amp->found_inf is set.  The deciding kernel
+  // (`amp_decide`, the engine's first update of the step, which has `entry_barrier`) carries amp->overflow in its
+  // AG_ARRIVE flag, ORs every rank's bit and writes the decision.
+  AmpState* amp;
+  uint32_t amp_decide;
 };
+
+// AG_ARRIVE flag encoding: (epoch << 1) | overflow bit of the sender (0 unless it is the deciding kernel).
+DEAR_HD uint32_t arrive_flag(uint32_t epoch, uint32_t overflow) { return (epoch << 1) | (overflow ? 1u : 0u); }
 
 // General ops on a symmetric staging buffer.
 enum GenOp : int {

@@ -146,6 +146,15 @@ __device__ __forceinline__ bool grid_arrive_is_last(uint32_t* counter) {
   return s_is_last != 0;
 }
 
+// true when none of f[0..N) is inf or NaN (dynamic loss scaling's overflow test)
+template <int N>
+__device__ __forceinline__ bool all_finite(const float* f) {
+  bool ok = true;
+#pragma unroll
+  for (int i = 0; i < N; ++i) ok &= isfinite(f[i]);
+  return ok;
+}
+
 // ----------------------------------------------------------------------------
 // element helpers
 // ----------------------------------------------------------------------------

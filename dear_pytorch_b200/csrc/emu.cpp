@@ -68,6 +68,13 @@ void rs_impl(const RSParams& p) {
   const uint32_t e8 = e << 8;                    // RS_READY = (epoch << 8) | stripes published, like the device kernels
   wait_all(sig_local, ch_done, e - 1, p.world, p.timeout_ns, p.status, ST_TIMEOUT_RS_DONE);
   const uint64_t off = uint64_t(p.rank) * p.shard_elems;
+  // 1/P (and 1/S of a static loss scale), times 1/scale of a dynamic one; a non-finite output sets amp->overflow
+  const float scale = p.amp ? p.scale * (1.f / p.amp->scale) : p.scale;
+  bool bad = false;
+  auto put = [&](uint64_t i, float v) {
+    p.out[i] = v;
+    if (p.amp && !std::isfinite(v)) bad = true;
+  };
   if (p.nstripes >= 1 && p.stripe_bytes > 0 && (p.pieces != nullptr || p.nstripes > 1)) {
     // stripe-pipelined variant (rs_pipe.cu): stripe k of every shard is packed from the stripe-major work list and
     // published; stripe k of my shard is reduced once every peer has published it
@@ -90,9 +97,10 @@ void rs_impl(const RSParams& p) {
       for (uint64_t i = lo; i < hi; ++i) {
         float acc = 0.f;
         for (int q = 0; q < p.world; ++q) acc += ld<T>(p.grad.ptr[q], off + i);   // fixed order
-        p.out[i] = acc * p.scale;
+        put(i, acc * scale);
       }
     }
+    if (bad) __atomic_fetch_or(&p.amp->overflow, 1u, __ATOMIC_RELAXED);
     signal_all(p.sig, ch_done, p.rank, p.world, e);
     *epoch_p = e;
     return;
@@ -107,8 +115,16 @@ void rs_impl(const RSParams& p) {
       const uint64_t off2 = uint64_t(tile - sg.tile_begin) * kPackTileBytes;
       const uint64_t left = sg.nbytes - off2;
       const uint32_t nb = left < kPackTileBytes ? uint32_t(left) : kPackTileBytes;
-      if (sg.flags & SEG_ZERO_FILL) std::memset(bucket + sg.dst_off + off2, 0, nb);
-      else if (sg.src != nullptr) std::memcpy(bucket + sg.dst_off + off2, reinterpret_cast<const char*>(sg.src) + off2, nb);
+      if (sg.flags & SEG_ZERO_FILL) {
+        std::memset(bucket + sg.dst_off + off2, 0, nb);
+      } else if (sg.src != nullptr && direct) {
+        // fp32, one rank: the pack writes the reduced shard, so it applies the factor the reduction would have
+        const float* src = reinterpret_cast<const float*>(reinterpret_cast<const char*>(sg.src) + off2);
+        const uint64_t o = (sg.dst_off + off2) / sizeof(float);
+        for (uint32_t k = 0; k < nb / sizeof(float); ++k) put(o + k, src[k] * scale);
+      } else if (sg.src != nullptr) {
+        std::memcpy(bucket + sg.dst_off + off2, reinterpret_cast<const char*>(sg.src) + off2, nb);
+      }
     }
   }
   signal_all(p.sig, ch_ready, p.rank, p.world, e8 | kAllStripes);
@@ -116,8 +132,9 @@ void rs_impl(const RSParams& p) {
   for (uint64_t i = 0; i < p.shard_elems && !direct; ++i) {
     float acc = 0.f;
     for (int q = 0; q < p.world; ++q) acc += ld<T>(p.grad.ptr[q], off + i);   // fixed order
-    p.out[i] = acc * p.scale;
+    put(i, acc * scale);
   }
+  if (bad) __atomic_fetch_or(&p.amp->overflow, 1u, __ATOMIC_RELAXED);
   signal_all(p.sig, ch_done, p.rank, p.world, e);
   *epoch_p = e;
 }
@@ -129,25 +146,38 @@ void ag_impl(const AGParams& p) {
   const uint32_t ch_pushed = bucket_channel(p.bucket, AG_PUSHED);
   uint32_t* epoch_p = p.ctrl + ch_arrive;
   const uint32_t e = *epoch_p + 1;
+  uint32_t found_inf = 0;
   if (p.entry_barrier) {
-    signal_all(p.sig, ch_arrive, p.rank, p.world, e);
-    wait_all(sig_local, ch_arrive, e, p.world, p.timeout_ns, p.status, ST_TIMEOUT_AG_ARRIVE);
+    // the deciding kernel's flags carry every rank's overflow bit (arrive_flag); OR them in rank order
+    const uint32_t ov = p.amp_decide ? p.amp->overflow : 0u;
+    signal_all(p.sig, ch_arrive, p.rank, p.world, arrive_flag(e, ov));
+    wait_all(sig_local, ch_arrive, arrive_flag(e, 0), p.world, p.timeout_ns, p.status, ST_TIMEOUT_AG_ARRIVE);
+    if (p.amp_decide) {
+      for (int r = 0; r < p.world; ++r) found_inf |= flag_load_acquire(flag_at(sig_local, ch_arrive, r)) & 1u;
+      p.amp->found_inf = found_inf;
+      amp_update_scale(p.amp, found_inf != 0);
+      if (!found_inf) p.amp->applied += 1;
+      p.amp->overflow = 0;
+    }
   }
+  if (p.amp && !p.amp_decide) found_inf = p.amp->found_inf;
+  const bool upd = p.do_update && !found_inf;      // a skipped step is a pure all-gather of the unchanged shard
+  const bool first_step = (p.amp && p.step_ctr) ? *p.step_ctr == 0 : p.first_step != 0;
   const uint64_t off = uint64_t(p.rank) * p.shard_elems;
   const bool has_mom = p.mom_shard != nullptr;
-  const bool adam = p.adam && p.do_update;
+  const bool adam = p.adam && upd;
   const uint32_t t_step = (adam && p.step_ctr) ? *p.step_ctr + 1 : 1;
   for (uint64_t i = 0; i < p.shard_elems; ++i) {
     float pv = p.master_shard ? p.master_shard[i] : ld<T>(p.param.ptr[p.rank], off + i);
-    if (p.do_update) {
+    if (upd) {
       const HyperSeg& h = p.hyper[p.nhyper == 1 ? 0 : find_hyper(p.hyper, p.nhyper, off + i)];
       if (adam) {
         const float bc1 = 1.f - std::pow(h.momentum, float(t_step));
         const float sqrt_bc2 = std::sqrt(1.f - std::pow(h.beta2, float(t_step)));
         pv = adam_update(pv, p.grad_shard[i], p.mom_shard[i], p.var_shard[i], h, bc1, sqrt_bc2);
       } else {
-        float mv = (has_mom && !p.first_step) ? p.mom_shard[i] : 0.f;
-        pv = sgd_update(pv, p.grad_shard[i], mv, h, p.first_step != 0, has_mom);
+        float mv = (has_mom && !first_step) ? p.mom_shard[i] : 0.f;
+        pv = sgd_update(pv, p.grad_shard[i], mv, h, first_step, has_mom);
         if (has_mom && h.momentum > 0.f) p.mom_shard[i] = mv;
       }
       if (p.master_shard) p.master_shard[i] = pv;
@@ -158,7 +188,7 @@ void ag_impl(const AGParams& p) {
   signal_all(p.sig, ch_pushed, p.rank, p.world, e);
   wait_all(sig_local, ch_pushed, e, p.world, p.timeout_ns, p.status, ST_TIMEOUT_AG_PUSHED);
   *epoch_p = e;
-  if (p.do_update && p.step_ctr) *p.step_ctr = *p.step_ctr + 1;
+  if (upd && p.step_ctr) *p.step_ctr = *p.step_ctr + 1;
 }
 
 template <typename T>

@@ -39,7 +39,9 @@ namespace dear {
 // ----------------------------------------------------------------------------
 constexpr int kPackVecPerThread = kPackTileBytes / 16 / kThreads;   // 8 x 128-bit per thread per tile
 
-template <typename T, int W, bool MC>
+// AMP: dynamic loss scaling (p.amp != nullptr) — divide by the device-resident scale and test every written value for
+// finiteness.  A separate instantiation, so the static path compiles to exactly the work it did without a scaler.
+template <typename T, int W, bool MC, bool AMP>
 __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
   using Tr = ElemTraits<T>;
   constexpr int EV = Tr::kPerVec;
@@ -58,6 +60,9 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
   // so the pack writes the fp32 shard (== the whole bucket) directly and the pull phase disappears.
   const bool direct = (W == 1) && p.direct_out;
   const bool direct16 = direct && sizeof(T) == 2;
+  // 1/P (and 1/S of a static loss scale), times 1/scale of a dynamic one
+  const float scale = AMP ? p.scale * (1.f / *reinterpret_cast<volatile float*>(&p.amp->scale)) : p.scale;
+  bool bad = false;                               // AMP: this thread wrote a non-finite value
 
   // (0) my bucket may still be read by a peer's previous reduce-scatter.
   wait_all_peers(sig_local, ch_done, e - 1, world, p.timeout_ns, p.status, ST_TIMEOUT_RS_DONE);
@@ -99,13 +104,19 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
           if (v < nvec) {
             float f[8];
             Tr::unpack(r[k], f);
+#pragma unroll
+            for (int x = 0; x < 8; ++x) f[x] *= scale;
+            if (AMP) bad |= !all_finite<8>(f);
             float4* o4 = reinterpret_cast<float4*>(o + size_t(v) * 8);
-            o4[0] = make_float4(f[0] * p.scale, f[1] * p.scale, f[2] * p.scale, f[3] * p.scale);
-            o4[1] = make_float4(f[EV - 4] * p.scale, f[EV - 3] * p.scale, f[EV - 2] * p.scale, f[EV - 1] * p.scale);
+            o4[0] = make_float4(f[0], f[1], f[2], f[3]);
+            o4[1] = make_float4(f[EV - 4], f[EV - 3], f[EV - 2], f[EV - 1]);
           }
         }
-        for (uint32_t b = (nvec << 4) + tid * 2; b < nb; b += kThreads * 2)
-          o[b >> 1] = zero ? 0.f : Tr::from_raw16(*reinterpret_cast<const uint16_t*>(s + b)) * p.scale;
+        for (uint32_t b = (nvec << 4) + tid * 2; b < nb; b += kThreads * 2) {
+          const float x = zero ? 0.f : Tr::from_raw16(*reinterpret_cast<const uint16_t*>(s + b)) * scale;
+          if (AMP) bad |= !isfinite(x);
+          o[b >> 1] = x;
+        }
         continue;
       }
       if (sg.flags & SEG_ZERO_FILL) {
@@ -124,6 +135,26 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
         for (int k = 0; k < kPackVecPerThread; ++k) {
           const uint32_t v = tid + k * kThreads;
           if (v < nvec) r[k] = ld_stream(s + (size_t(v) << 4));
+        }
+        if (direct) {
+          // fp32 gradients, one GPU: the pack writes the fp32 shard, so it applies the factor the pull phase would have
+#pragma unroll
+          for (int k = 0; k < kPackVecPerThread; ++k) {
+            const uint32_t v = tid + k * kThreads;
+            if (v < nvec) {
+              float f[4] = {__uint_as_float(r[k].x) * scale, __uint_as_float(r[k].y) * scale,
+                            __uint_as_float(r[k].z) * scale, __uint_as_float(r[k].w) * scale};
+              if (AMP) bad |= !all_finite<4>(f);
+              st_stream(d + (size_t(v) << 4),
+                        make_uint4(__float_as_uint(f[0]), __float_as_uint(f[1]), __float_as_uint(f[2]), __float_as_uint(f[3])));
+            }
+          }
+          for (uint32_t b = (nvec << 4) + tid * 4; b < nb; b += kThreads * 4) {
+            const float x = *reinterpret_cast<const float*>(s + b) * scale;
+            if (AMP) bad |= !isfinite(x);
+            *reinterpret_cast<float*>(d + b) = x;
+          }
+          continue;
         }
 #pragma unroll
         for (int k = 0; k < kPackVecPerThread; ++k) {
@@ -150,7 +181,6 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
     const uint64_t nvec = p.shard_elems / EV;
     const uint64_t shard_byte_off = uint64_t(p.rank) * p.shard_elems * sizeof(T);
     const uint64_t gstride = uint64_t(gridDim.x) * kThreads;
-    const float scale = p.scale;
     if (MC) {
       const char* mc = reinterpret_cast<const char*>(p.mc_grad) + shard_byte_off;
       constexpr int U = 8;
@@ -169,6 +199,7 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
             Tr::unpack(r[u], f);
 #pragma unroll
             for (int k = 0; k < EV; ++k) f[k] *= scale;
+            if (AMP) bad |= !all_finite<EV>(f);
             float4* o = reinterpret_cast<float4*>(p.out + v * EV);
             o[0] = make_float4(f[0], f[1], f[2], f[3]);
             if (EV == 8) o[1] = make_float4(f[EV - 4], f[EV - 3], f[EV - 2], f[EV - 1]);
@@ -205,10 +236,12 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
 #pragma unroll
               for (int k = 0; k < EV; ++k) acc[k] += f[k];
             }
+#pragma unroll
+            for (int k = 0; k < EV; ++k) acc[k] *= scale;
+            if (AMP) bad |= !all_finite<EV>(acc);
             float4* o = reinterpret_cast<float4*>(p.out + v * EV);
-            o[0] = make_float4(acc[0] * scale, acc[1] * scale, acc[2] * scale, acc[3] * scale);
-            if (EV == 8)
-              o[1] = make_float4(acc[EV - 4] * scale, acc[EV - 3] * scale, acc[EV - 2] * scale, acc[EV - 1] * scale);
+            o[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+            if (EV == 8) o[1] = make_float4(acc[EV - 4], acc[EV - 3], acc[EV - 2], acc[EV - 1]);
           }
         }
       }
@@ -237,15 +270,21 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
         for (int u = 0; u < U; ++u) {
           const uint64_t v = v0 + u * gstride;
           if (v < nvec) {
+#pragma unroll
+            for (int k = 0; k < EV; ++k) acc[u][k] *= scale;
+            if (AMP) bad |= !all_finite<EV>(acc[u]);
             float4* o = reinterpret_cast<float4*>(p.out + v * EV);
-            o[0] = make_float4(acc[u][0] * scale, acc[u][1] * scale, acc[u][2] * scale, acc[u][3] * scale);
-            if (EV == 8)
-              o[1] = make_float4(acc[u][EV - 4] * scale, acc[u][EV - 3] * scale, acc[u][EV - 2] * scale,
-                                 acc[u][EV - 1] * scale);
+            o[0] = make_float4(acc[u][0], acc[u][1], acc[u][2], acc[u][3]);
+            if (EV == 8) o[1] = make_float4(acc[u][EV - 4], acc[u][EV - 3], acc[u][EV - 2], acc[u][EV - 1]);
           }
         }
       }
     }
+  }
+
+  // AMP: one atomic per CTA into this rank's overflow word (read by the step's deciding Kernel B)
+  if (AMP) {
+    if (__syncthreads_or(bad) && tid == 0) atomicOr(&p.amp->overflow, 1u);
   }
 
   // (5) tell every peer I am done reading its bucket; advance the epoch.
@@ -300,13 +339,36 @@ __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
   const HyperSeg* hyper = hyper_smem ? s_hyper : p.hyper;
 
   // (0) nobody may overwrite a peer's parameters before that peer finished the
-  // backward pass that still reads them: rendezvous at kernel entry.
+  // backward pass that still reads them: rendezvous at kernel entry.  With a dynamic loss scale the deciding kernel's
+  // flags carry every rank's overflow bit: each CTA ORs them (fixed rank order), so all ranks reach the same decision.
+  AmpState* const amp = p.amp;
+  uint32_t found_inf = 0;
   if (p.entry_barrier) {
-    if (blockIdx.x == 0) signal_all_peers(p.sig, ch_arrive, p.rank, world, e);
-    wait_all_peers(sig_local, ch_arrive, e, world, p.timeout_ns, p.status, ST_TIMEOUT_AG_ARRIVE);
+    if (blockIdx.x == 0) {
+      const uint32_t ov = (p.amp_decide && tid < world) ? *reinterpret_cast<volatile uint32_t*>(&amp->overflow) : 0u;
+      signal_all_peers(p.sig, ch_arrive, p.rank, world, arrive_flag(e, ov));
+    }
+    wait_all_peers(sig_local, ch_arrive, arrive_flag(e, 0), world, p.timeout_ns, p.status, ST_TIMEOUT_AG_ARRIVE);
+    if (p.amp_decide) {
+      const uint32_t bit = tid < world ? (ld_acquire_sys(flag_at(sig_local, ch_arrive, tid)) & 1u) : 0u;
+      found_inf = __syncthreads_or(bit) ? 1u : 0u;
+      if (blockIdx.x == 0 && tid == 0) {
+        amp->found_inf = found_inf;
+        amp_update_scale(amp, found_inf != 0);
+        if (!found_inf) amp->applied += 1;
+        amp->overflow = 0;            // the next step's reduce-scatters are stream-ordered after this kernel
+      }
+    }
   } else {
     __syncthreads();
   }
+  // the step's other update kernels follow the deciding one on the all-gather stream(s)
+  if (amp != nullptr && !p.amp_decide) found_inf = *reinterpret_cast<volatile uint32_t*>(&amp->found_inf);
+  // a skipped step is a pure all-gather of the unchanged shard: same flag rounds, gradient bucket still zeroed
+  const bool upd = p.do_update && !found_inf;
+  // with a dynamic loss scale the host cannot know which update is the first one applied: count on the device
+  const bool first_step = (amp != nullptr && p.step_ctr != nullptr) ? *reinterpret_cast<volatile uint32_t*>(p.step_ctr) == 0
+                                                                     : p.first_step != 0;
 
   // (1) update my shard and push it into every rank's parameter bucket.
   {
@@ -315,7 +377,7 @@ __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
     const uint64_t gstride = uint64_t(gridDim.x) * kThreads;
     const char* local_param = reinterpret_cast<const char*>(p.param.ptr[p.rank]);
     const bool has_mom = p.mom_shard != nullptr;
-    const bool load_mom = has_mom && (ADAM || !p.first_step) && p.do_update;
+    const bool load_mom = has_mom && (ADAM || !first_step) && upd;
     // Adam bias corrections come from a device-resident update counter (graph replay safe)
     const uint32_t t_step = (ADAM && p.step_ctr != nullptr) ? *reinterpret_cast<volatile uint32_t*>(p.step_ctr) + 1 : 1;
     for (uint64_t v0 = uint64_t(blockIdx.x) * kThreads + tid; v0 < nvec; v0 += gstride * U) {
@@ -331,14 +393,14 @@ __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
           } else {
             Tr::unpack(*reinterpret_cast<const uint4*>(local_param + (shard_elem_off + v * EV) * sizeof(T)), pv[u]);
           }
-          if (p.do_update) ld_f32x(p.grad_shard, v, EV, gv[u]);
+          if (upd) ld_f32x(p.grad_shard, v, EV, gv[u]);
           if (load_mom) {
             ld_f32x(p.mom_shard, v, EV, mv[u]);
           } else {
 #pragma unroll
             for (int k = 0; k < EV; ++k) mv[u][k] = 0.f;
           }
-          if (ADAM && p.do_update) ld_f32x(p.var_shard, v, EV, vv[ADAM ? u : 0]);
+          if (ADAM && upd) ld_f32x(p.var_shard, v, EV, vv[ADAM ? u : 0]);
         }
       }
       // ---- update + stores ----
@@ -347,7 +409,7 @@ __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
         const uint64_t v = v0 + u * gstride;
         if (v < nvec) {
           const uint64_t ge = shard_elem_off + v * EV;     // element offset within the bucket
-          if (p.do_update) {
+          if (upd) {
             const HyperSeg h = hyper[p.nhyper == 1 ? 0 : find_hyper(hyper, p.nhyper, ge)];
             if (ADAM) {
               const float bc1 = 1.f - powf(h.momentum, float(t_step));
@@ -360,7 +422,7 @@ __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
             } else {
 #pragma unroll
               for (int k = 0; k < EV; ++k)
-                pv[u][k] = sgd_update(pv[u][k], gv[u][k], mv[u][k], h, p.first_step != 0, has_mom);
+                pv[u][k] = sgd_update(pv[u][k], gv[u][k], mv[u][k], h, first_step, has_mom);
               if (has_mom && h.momentum > 0.f) st_f32x(p.mom_shard, v, EV, mv[u]);
             }
             if (p.master_shard != nullptr) st_f32x(p.master_shard, v, EV, pv[u]);
@@ -402,7 +464,7 @@ __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
     if (tid == 0) {
       *cnt_exit = 0;
       *epoch_p = e;
-      if (p.do_update && p.step_ctr != nullptr) *p.step_ctr = *p.step_ctr + 1;
+      if (upd && p.step_ctr != nullptr) *p.step_ctr = *p.step_ctr + 1;
     }
   }
 }
@@ -564,15 +626,21 @@ static void check_launch(const char* what) {
     throw std::runtime_error(std::string("dear: launch of ") + what + " failed: " + cudaGetErrorString(err));
 }
 
+template <typename T, bool MC, bool AMP>
+static void launch_rs_wa(const RSParams& p, int grid, cudaStream_t s) {
+  switch (p.world) {
+    case 1: rs_kernel<T, 1, MC, AMP><<<grid, kThreads, 0, s>>>(p); break;
+    case 2: rs_kernel<T, 2, MC, AMP><<<grid, kThreads, 0, s>>>(p); break;
+    case 4: rs_kernel<T, 4, MC, AMP><<<grid, kThreads, 0, s>>>(p); break;
+    case 8: rs_kernel<T, 8, MC, AMP><<<grid, kThreads, 0, s>>>(p); break;
+    default: rs_kernel<T, 0, MC, AMP><<<grid, kThreads, 0, s>>>(p); break;
+  }
+}
+
 template <typename T, bool MC>
 static void launch_rs_w(const RSParams& p, int grid, cudaStream_t s) {
-  switch (p.world) {
-    case 1: rs_kernel<T, 1, MC><<<grid, kThreads, 0, s>>>(p); break;
-    case 2: rs_kernel<T, 2, MC><<<grid, kThreads, 0, s>>>(p); break;
-    case 4: rs_kernel<T, 4, MC><<<grid, kThreads, 0, s>>>(p); break;
-    case 8: rs_kernel<T, 8, MC><<<grid, kThreads, 0, s>>>(p); break;
-    default: rs_kernel<T, 0, MC><<<grid, kThreads, 0, s>>>(p); break;
-  }
+  if (p.amp != nullptr) launch_rs_wa<T, MC, true>(p, grid, s);
+  else launch_rs_wa<T, MC, false>(p, grid, s);
 }
 
 void launch_rs(const RSParams& p, int grid, cudaStream_t s) {

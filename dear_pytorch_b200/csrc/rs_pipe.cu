@@ -114,7 +114,8 @@ __device__ __forceinline__ uint32_t first_chunk(uint32_t k, uint64_t stripe_byte
   return (blockIdx.x + gridDim.x - before) % gridDim.x;
 }
 
-template <typename T>
+// AMP: dynamic loss scaling (p.amp != nullptr), see rs_kernel in kernels.cu.
+template <typename T, bool AMP>
 __global__ void __launch_bounds__(kPipeThreads, 1) rs_pipe_kernel(const RSParams p) {
   using Tr = ElemTraits<T>;
   constexpr int EV = Tr::kPerVec;
@@ -154,6 +155,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) rs_pipe_kernel(const RSParams
   const uint32_t K = p.nstripes;
   const uint64_t cs = p.stripe_bytes;
   const uint64_t my_shard_off = uint64_t(p.rank) * SB;
+  bool bad = false;                               // AMP: this thread wrote a non-finite value
 
   if (tid >= 32 + kReduceThreads) {
     // ================================ PACK ================================
@@ -223,7 +225,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) rs_pipe_kernel(const RSParams
   } else {
     // =============================== REDUCE ===============================
     const int rtid = tid - 32;
-    const float scale = p.scale;
+    const float scale = AMP ? p.scale * (1.f / *reinterpret_cast<volatile float*>(&p.amp->scale)) : p.scale;
     int s = 0;
     uint32_t ph = 0;
     bool ok = true;
@@ -265,14 +267,21 @@ __global__ void __launch_bounds__(kPipeThreads, 1) rs_pipe_kernel(const RSParams
         for (int i = 0; i < kRedVecs; ++i) {
           const uint32_t v = rtid + i * kReduceThreads;
           if (v < nvec) {
+#pragma unroll
+            for (int x = 0; x < EV; ++x) acc[i][x] *= scale;
+            if (AMP) bad |= !all_finite<EV>(acc[i]);
             float4* o = reinterpret_cast<float4*>(out + size_t(v) * EV);
-            o[0] = make_float4(acc[i][0] * scale, acc[i][1] * scale, acc[i][2] * scale, acc[i][3] * scale);
-            if (EV == 8)
-              o[1] = make_float4(acc[i][EV - 4] * scale, acc[i][EV - 3] * scale, acc[i][EV - 2] * scale, acc[i][EV - 1] * scale);
+            o[0] = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+            if (EV == 8) o[1] = make_float4(acc[i][EV - 4], acc[i][EV - 3], acc[i][EV - 2], acc[i][EV - 1]);
           }
         }
       }
     }
+  }
+
+  // AMP: one atomic per CTA into this rank's overflow word (every role reaches this point)
+  if (AMP) {
+    if (__syncthreads_or(bad) && tid == 0) atomicOr(&p.amp->overflow, 1u);
   }
 
   // (end) tell every peer I am done reading its bucket; advance the epoch.
@@ -286,18 +295,24 @@ __global__ void __launch_bounds__(kPipeThreads, 1) rs_pipe_kernel(const RSParams
   }
 }
 
-static bool g_pipe_attr_set[3] = {false, false, false};
+static bool g_pipe_attr_set[6] = {false, false, false, false, false, false};
 
-template <typename T>
-static void launch_pipe_t(const RSParams& p, int grid, cudaStream_t s, int slot) {
+template <typename T, bool AMP>
+static void launch_pipe_ta(const RSParams& p, int grid, cudaStream_t s, int slot) {
   constexpr int smem = kPipeStages * kPipeChunk;
   if (!g_pipe_attr_set[slot]) {
-    cudaError_t err = cudaFuncSetAttribute(rs_pipe_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t err = cudaFuncSetAttribute(rs_pipe_kernel<T, AMP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (err != cudaSuccess)
       throw std::runtime_error(std::string("dear: cannot reserve shared memory for rs_pipe_kernel: ") + cudaGetErrorString(err));
     g_pipe_attr_set[slot] = true;
   }
-  rs_pipe_kernel<T><<<grid, kPipeThreads, smem, s>>>(p);
+  rs_pipe_kernel<T, AMP><<<grid, kPipeThreads, smem, s>>>(p);
+}
+
+template <typename T>
+static void launch_pipe_t(const RSParams& p, int grid, cudaStream_t s, int slot) {
+  if (p.amp != nullptr) launch_pipe_ta<T, true>(p, grid, s, 3 + slot);
+  else launch_pipe_ta<T, false>(p, grid, s, slot);
 }
 
 void launch_rs_pipe(const RSParams& p, int grid, cudaStream_t s) {

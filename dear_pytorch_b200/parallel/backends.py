@@ -68,6 +68,7 @@ class _BackendBase:
         self.var_shard: List[Optional[torch.Tensor]] = [None] * nb       # Adam exp_avg_sq
         self.hyper: List[Optional[HyperSpec]] = [None] * nb
         self.grad_scale = 1.0
+        self.amp: Optional[torch.Tensor] = None     # dynamic loss scaler state (parallel/grad_scaler.py), engine-owned
 
     # -- shard state ------------------------------------------------------------------
     def _alloc_shards(self):
@@ -112,6 +113,10 @@ class _BackendBase:
     def stream_key(self, g: int) -> int:
         """Buckets with the same key share one communication stream (ordering domain)."""
         return 0
+
+    def set_amp(self, state: Optional[torch.Tensor]) -> None:
+        """Dynamic loss scaling: ``state`` is the engine's int32[9] AmpState (csrc/dear_common.h), or None."""
+        self.amp = state
 
 
 # =====================================================================================
@@ -186,11 +191,23 @@ class NativeBackend(_BackendBase):
         bs, li = self.where[g]
         bs.reduce_scatter(li, pack)
 
+    def set_amp(self, state):
+        self.amp = state
+        for bs in self.sets.values():
+            bs.set_amp(state)
+
     def allgather_update(self, g, do_update=True, first_step=False, zero_grad=False):
         bs, li = self.where[g]
         # the first bucket of every set carries the entry rendezvous: nobody overwrites a
         # peer's parameters before that peer has finished its backward pass.
-        bs.allgather_update(li, do_update, first_step, self._first_in_set[id(bs)] == g, zero_grad)
+        entry = self._first_in_set[id(bs)] == g
+        # dynamic loss scaling: bucket 0's update decides for the whole step.  With several dtype sets it waits for every
+        # set's reduce-scatters, and the other sets' first updates wait for it.
+        decide = self.amp is not None and g == 0 and do_update
+        if self.amp is not None and entry and len(self.sets) > 1:
+            for other in (self.sets.values() if decide else (self.where[0][0],)):
+                bs.join(other)
+        bs.allgather_update(li, do_update, first_step, entry, zero_grad, decide)
 
     def fence(self):
         for bs in self.sets.values():
@@ -257,6 +274,26 @@ class TorchBackend(_BackendBase):
     def set_step(self, t: int):
         self._t = int(t)
 
+    def set_amp(self, state):
+        self.amp = state
+        self._overflow = None if state is None else torch.zeros((), dtype=torch.float32, device=self.device)
+        self._skip = False
+
+    def _amp_decide(self):
+        """One decision per step: did any rank see a non-finite reduced gradient?  Then skip every bucket's update;
+        the scale and growth tracker follow torch.amp.GradScaler (torch._amp_update_scale_)."""
+        found = self._overflow.reshape(1).clone()
+        if self.world > 1:
+            dist.all_reduce(found, op=dist.ReduceOp.MAX, group=self.group)
+        st, f32 = self.amp, self.amp.view(torch.float32)
+        st[8] = st[3]
+        torch._amp_update_scale_(f32[2:3], st[3:4], found, float(f32[5]), float(f32[6]), int(st[7]))
+        self._skip = bool(found.item())
+        st[1] = int(self._skip)
+        if not self._skip:
+            st[4] += 1
+        self._overflow.zero_()
+
     def set_pack(self, g, src_ptrs, dst_off, nbytes, flags):
         pass    # gradients are accumulated straight into the bucket views
 
@@ -275,11 +312,18 @@ class TorchBackend(_BackendBase):
             else:
                 self._rs_out[g].copy_(self._gbuf[g])
             torch.mul(self._rs_out[g].float(), self.grad_scale / self.world, out=self.grad_shard[g])
+            if self.amp is not None:
+                self.grad_shard[g].mul_(self.amp.view(torch.float32)[2].reciprocal())
+                torch.maximum(self._overflow, (~torch.isfinite(self.grad_shard[g])).any().float(), out=self._overflow)
             self._gbuf[g].zero_()
         self._n_launch += 3
 
     @torch.no_grad()
     def _sgd_shard(self, g, first_step):
+        if self.amp is not None:
+            if self._skip:
+                return
+            first_step = self._t == 0             # counts applied updates only
         b = self.plan.buckets[g]
         lo, hi = self.rank * b.shard_numel, (self.rank + 1) * b.shard_numel
         master = self.master_shard[g]
@@ -324,6 +368,8 @@ class TorchBackend(_BackendBase):
         b = self.plan.buckets[g]
         lo = self.rank * b.shard_numel
         with self._on_comm_stream():
+            if do_update and g == 0 and self.amp is not None:
+                self._amp_decide()
             if do_update:
                 self._sgd_shard(g, first_step)
             if self.master_shard[g] is not None:
@@ -334,7 +380,7 @@ class TorchBackend(_BackendBase):
                 dist.all_gather_into_tensor(self._pbuf[g], src, group=self.group)
             else:
                 self._pbuf[g][lo:lo + b.shard_numel].copy_(src)
-            if do_update and g == len(self.plan.buckets) - 1:
+            if do_update and g == len(self.plan.buckets) - 1 and not (self.amp is not None and self._skip):
                 self._t += 1
             if self.cuda:
                 self.ag_done[g].record(self.stream)

@@ -73,6 +73,7 @@ class DearEngine:
         self.num_nearby_layers = num_nearby_layers
         self._mom_initialised = False
         self.num_updates = 0               # parameter updates applied so far (Adam bias correction)
+        self.amp: Optional[torch.Tensor] = None   # dynamic loss scaler state (attach_scaler), survives re-bucketing
         self.flush_callbacks = []          # run by flush(): deferred work of the training loop (TrainStep.finish)
         if int(backward_passes_per_step) < 1:
             raise ValueError("backward_passes_per_step must be >= 1")
@@ -173,6 +174,7 @@ class DearEngine:
         self.backend = self._make_backend()
         be = self.backend
         be.set_grad_scale(1.0 / getattr(self, "loss_scale", 1.0))
+        be.set_amp(self.amp)
         self.steal = be.steal_grads
         self._param_view: Dict[nn.Parameter, torch.Tensor] = {}
         self._grad_view: Dict[nn.Parameter, torch.Tensor] = {}
@@ -203,7 +205,7 @@ class DearEngine:
         be.init_master_shards()
         if carry is not None:
             self._restore_state(carry)
-        be.set_step(self.num_updates)
+        self.set_step(self.num_updates)
         nb = len(plan.buckets)
         self._n_params = [len(b.slots) for b in plan.buckets]
         self._arrived = [[False] * n for n in self._n_params]
@@ -466,9 +468,65 @@ class DearEngine:
         1/P of the reduce-scatter epilogue — no extra pass over the gradients.  Call it before ``backward()``."""
         if scale <= 0:
             raise ValueError("loss scale must be positive")
+        if self.amp is not None:
+            raise ValueError("this optimizer has a dynamic loss scaler (GradScaler); a static loss scale cannot be combined "
+                             "with it")
         self.loss_scale = float(scale)
         if self.backend is not None:
             self.backend.set_grad_scale(1.0 / self.loss_scale)
+
+    # ------------------------------------------------------------------ dynamic loss scaling (GradScaler)
+    # AmpState words (csrc/dear_common.h): 0 overflow, 1 found_inf, 2 scale (f32), 3 growth tracker, 4 applied updates,
+    # 5 growth factor (f32), 6 backoff factor (f32), 7 growth interval, 8 growth tracker before the last step's rule
+    _AMP_F32 = {"scale": 2, "growth_factor": 5, "backoff_factor": 6}
+    _AMP_I32 = {"growth_tracker": 3, "applied": 4, "growth_interval": 7, "prev_growth_tracker": 8}
+
+    def set_step(self, t: int):
+        """Number of updates applied so far, set from the host (build, re-bucketing, checkpoint resume): the kernels'
+        step counters and, with a scaler, its count of applied updates (the source of the step count from then on)."""
+        self.num_updates = int(t)
+        self.backend.set_step(self.num_updates)
+        if self.amp is not None:
+            self.write_scaler(applied=self.num_updates)
+
+    def attach_scaler(self, init_scale: float, growth_factor: float, backoff_factor: float, growth_interval: int):
+        """Switch to dynamic loss scaling: the kernels divide the reduced gradient by a device-resident scale, skip
+        the update of a step in which any rank saw a non-finite value, and adjust the scale like torch's GradScaler."""
+        if getattr(self, "loss_scale", None) is not None:
+            raise ValueError("this optimizer has a static loss_scale; a dynamic loss scaler (GradScaler) cannot be "
+                             "combined with it")
+        if self.amp is not None:
+            raise ValueError("this optimizer already has a GradScaler")
+        self.synchronize(host=False)
+        self.amp = torch.zeros(9, dtype=torch.int32, device=self.device)
+        self.write_scaler(scale=init_scale, growth_factor=growth_factor, backoff_factor=backoff_factor,
+                          growth_interval=growth_interval, growth_tracker=0, prev_growth_tracker=0,
+                          applied=self.num_updates)
+        self.backend.set_amp(self.amp)
+
+    def scaler_scale(self) -> torch.Tensor:
+        """The device scale as a 0-dim fp32 tensor, usable by the current stream (ordered after the last update)."""
+        self.synchronize(host=False)
+        return self.amp.view(torch.float32)[2]
+
+    def write_scaler(self, **fields):
+        """Set AmpState fields from the host, in current-stream order after every queued update."""
+        self.synchronize(host=False)
+        f32 = self.amp.view(torch.float32)
+        for k, v in fields.items():
+            if k in self._AMP_F32:
+                f32[self._AMP_F32[k]].fill_(float(v))
+            else:
+                self.amp[self._AMP_I32[k]].fill_(int(v))
+
+    def read_scaler(self) -> dict:
+        """Host copy of the AmpState fields (synchronises the host)."""
+        self.synchronize(host=True)
+        st = self.amp.cpu()
+        f32 = st.view(torch.float32)
+        out = {k: float(f32[i]) for k, i in self._AMP_F32.items()}
+        out.update({k: int(st[i]) for k, i in self._AMP_I32.items()})
+        return out
 
     def params_changed(self):
         """The parameter VALUES were overwritten from outside (``broadcast_parameters``, ``load_state_dict``,
@@ -585,6 +643,10 @@ class DearEngine:
         """Full (un-sharded) optimizer state per parameter name: momentum and fp32 master."""
         from ..utils.checkpoint import gather_sharded
         out = {"momentum": {}, "master": {}, "var": {}, "mom_init": self._mom_initialised, "num_updates": self.num_updates}
+        if self.amp is not None:
+            # skipped steps applied nothing: the device count of applied updates is the step count of the new buckets
+            applied = self.read_scaler()["applied"]
+            out.update(num_updates=applied, mom_init=applied > 0)
         for b in self.plan.buckets:
             g = b.index
             for kind, shard in (("momentum", self.backend.mom_shard[g]), ("master", self.backend.master_shard[g]),

@@ -72,7 +72,7 @@ def optimizer_state_dict(optimizer) -> dict:
         d["params"] = [index[p] for p in g["params"]]
         groups.append(d)
     return {"state": state, "param_groups": groups,
-            "dear": {"num_steps": eng.num_steps, "num_updates": eng.num_updates, "policy": eng.plan.policy,
+            "dear": {"num_steps": eng.num_steps, "num_updates": carry["num_updates"], "policy": eng.plan.policy,
                      "world": eng.world}}
 
 
@@ -117,8 +117,11 @@ def load_optimizer_state_dict(optimizer, sd: dict) -> None:
         # through their hyper segment (DearEngine._adam_lag_adjust)
         carry["num_updates"] = max(adam_steps.values())
         eng._lag = {p: carry["num_updates"] - v for p, v in adam_steps.items() if v < carry["num_updates"]}
+    if eng.opt_kind == 0 and carry["mom_init"]:
+        # momentum buffers exist, so the next update is not the first one (a stock torch.optim.SGD state has no count)
+        carry["num_updates"] = max(carry["num_updates"], 1)
     eng._restore_state(carry)
-    eng.backend.set_step(eng.num_updates)
+    eng.set_step(eng.num_updates)
     eng._hyper_key = [None] * len(eng._hyper_key)
     eng.num_steps = int(meta.get("num_steps", eng.num_steps))
 

@@ -59,8 +59,9 @@ def _first_tensor(obj):
 
 class TrainStep:
     def __init__(self, model: torch.nn.Module, optimizer, loss_fn: Callable, autocast_dtype: Optional[torch.dtype] = None,
-                 use_graph: bool = False, graph_warmup: int = 3, overlap_update: bool = False):
+                 use_graph: bool = False, graph_warmup: int = 3, overlap_update: bool = False, scaler=None):
         self.model = model
+        self.scaler = scaler               # dear.GradScaler: back-propagate scaler.scale(loss) (dynamic loss scaling)
         self.opt = optimizer
         self.loss_fn = loss_fn
         self.autocast_dtype = autocast_dtype
@@ -88,7 +89,7 @@ class TrainStep:
         else:
             out = self.model(*inputs)
         loss = self.loss_fn(out, target)
-        loss.backward()
+        (self.scaler.scale(loss) if self.scaler is not None else loss).backward()
         return loss.detach()
 
     def _eager(self, *batch):

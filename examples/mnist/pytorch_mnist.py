@@ -63,7 +63,8 @@ def main(argv=None):
     ap.add_argument("--threshold", type=float, default=0.05, help="fusion threshold in MB (the net has 0.08 MB)")
     ap.add_argument("--use-mixed-precision", action="store_true", default=False,
                     help="autocast forward + scaled loss (reference: train_mixed_precision, pytorch_mnist.py:63-83)")
-    ap.add_argument("--loss-scale", type=float, default=128.0, help="static loss scale of the mixed-precision path")
+    ap.add_argument("--loss-scale", type=float, default=None,
+                    help="static loss scale of the mixed-precision path (default: dynamic, dear.GradScaler)")
     # parsed by the reference's example too, where only --use-adasum has an effect (the learning rate is then not scaled
     # by the number of ranks; the Horovod compression / Adasum / predivide arguments are commented out there,
     # examples/mnist/pytorch_mnist.py:207-235 of the reference)
@@ -103,27 +104,39 @@ def main(argv=None):
                 print("Train Epoch: {} [{}/{} ({:.0f}%)]\tLoss: {:.6f}".format(
                     epoch, batch_idx * len(data), len(train_sampler), 100.0 * batch_idx / len(train_loader), loss.item()))
 
+    scaler = hvd.GradScaler(optimizer) if (args.use_mixed_precision and args.loss_scale is None) else None
+
     def train_mixed_precision(epoch):
         """The reference's GradScaler loop (examples/mnist/pytorch_mnist.py:63-83): synchronize -> unscale ->
         ``with optimizer.skip_synchronize(): step``.  Here the gradients never surface as tensors (Kernel A consumes
-        them during back-propagation), so the un-scaling is a factor of the reduce-scatter epilogue
-        (``set_loss_scale``) instead of a pass over the gradients; the call sequence is kept."""
+        them during back-propagation), so the un-scaling is a factor of the reduce-scatter epilogue instead of a pass
+        over the gradients.  dear.GradScaler (default) keeps the reference's call sequence and scales dynamically on
+        the device; ``--loss-scale X`` runs a static scale (``set_loss_scale``)."""
         model.train()
         train_sampler.set_epoch(epoch)
-        optimizer.set_loss_scale(args.loss_scale)
+        if scaler is None:
+            optimizer.set_loss_scale(args.loss_scale)
         amp_dtype = torch.bfloat16 if (device.type == "cpu" or torch.cuda.is_bf16_supported()) else torch.float16
         for batch_idx, (data, target) in enumerate(train_loader):
             data, target = data.to(device), target.to(device)
             optimizer.zero_grad()
             with torch.autocast(device.type, dtype=amp_dtype):
                 loss = F.nll_loss(model(data).float(), target)
-            (loss * args.loss_scale).backward()
-            with optimizer.skip_synchronize():
-                optimizer.step()
+            if scaler is not None:
+                scaler.scale(loss).backward()
+                optimizer.synchronize()
+                scaler.unscale_(optimizer)
+                with optimizer.skip_synchronize():
+                    scaler.step(optimizer)
+                scaler.update()
+            else:
+                (loss * args.loss_scale).backward()
+                with optimizer.skip_synchronize():
+                    optimizer.step()
             if batch_idx % args.log_interval == 0 and hvd.rank() == 0:
                 print("Train Epoch: {} [{}/{} ({:.0f}%)]\tLoss: {:.6f}\tLoss Scale: {}".format(
                     epoch, batch_idx * len(data), len(train_sampler), 100.0 * batch_idx / len(train_loader), loss.item(),
-                    args.loss_scale))
+                    scaler.get_scale() if scaler is not None else args.loss_scale))
 
     def test():
         model.eval()
