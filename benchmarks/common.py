@@ -49,6 +49,9 @@ def add_common_args(ap):
     ap.add_argument("--optimizer", choices=["sgd", "adam", "adamw"], default="sgd",
                     help="adam/adamw: sharded Adam fused into the all-gather kernel (dear methods only)")
     ap.add_argument("--graph", type=int, default=0, help="capture the whole iteration in a CUDA graph")
+    ap.add_argument("--norm-clip", type=float, default=None,
+                    help="dear, dear-bo, dear-notf: clip the global gradient norm to this value (clip_grad_norm_ semantics, "
+                         "inside the fused kernels)")
     # flags of the reference's baseline drivers (horovod/, bytescheduler/, pytorch-ddp/ imagenet_benchmark.py)
     ap.add_argument("--fp16-allreduce", action="store_true", default=False,
                     help="--method horovod: fused buffers travel as fp16 (hvd.Compression.fp16)")
@@ -94,13 +97,14 @@ def wrap_optimizer(method, args, model, optimizer, profile_fn=None):
     if method == "single" or (world == 1 and not method.startswith("dear")):
         return model, optimizer
     if method == "dear":
-        return model, dear.DistributedOptimizer(optimizer, model, threshold=args.threshold, exclude_parts=args.exclude_parts)
+        return model, dear.DistributedOptimizer(optimizer, model, threshold=args.threshold, exclude_parts=args.exclude_parts,
+                                                norm_clip=args.norm_clip)
     if method == "dear-bo":
         return model, dear.DistributedOptimizer(optimizer, model, threshold=args.threshold, exclude_parts=args.exclude_parts,
-                                                bo_tuning=True)
+                                                bo_tuning=True, norm_clip=args.norm_clip)
     if method == "dear-notf":
         return model, dear.DistributedOptimizer(optimizer, model, threshold=None, num_nearby_layers=1,
-                                                exclude_parts=args.exclude_parts)
+                                                exclude_parts=args.exclude_parts, norm_clip=args.norm_clip)
     if method == "dear-naive":
         return model, variants.NaiveDistributedOptimizer(optimizer, model, exclude_parts=args.exclude_parts)
     if method == "dear-wt":

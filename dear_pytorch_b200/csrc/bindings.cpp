@@ -120,8 +120,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("pack_pieces", &BucketSet::pack_pieces, py::arg("bucket"))
       .def("allgather_update", &BucketSet::allgather_update, py::arg("bucket"), py::arg("do_update") = true,
            py::arg("first_step") = false, py::arg("entry_barrier") = true, py::arg("zero_grad") = false,
-           py::arg("amp_decide") = false)
+           py::arg("decide") = false)
       .def("set_amp", &BucketSet::set_amp, py::arg("state"))
+      .def("set_clip", &BucketSet::set_clip, py::arg("state"), py::arg("slots"))
       .def("join", &BucketSet::join, py::arg("other"))
       .def("fence_current_to_comm", &BucketSet::fence_current_to_comm)
       .def("wait_bucket", &BucketSet::wait_bucket)
@@ -150,6 +151,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("bias_gelu_forward", &dear::ln::bias_gelu_forward);
   m.def("bias_gelu_backward", &dear::ln::bias_gelu_backward);
 
+  // float32 elements of a ClipState for `nslots` buckets (BucketSet.set_clip); word 0 max_norm, 1 total_norm, 2 coef
+  m.def("clip_state_floats", [](int64_t nslots) { return static_cast<int64_t>(clip_state_floats(static_cast<uint32_t>(nslots))); });
   m.attr("OPT_SGD") = static_cast<int>(OPT_SGD);
   m.attr("OPT_ADAM") = static_cast<int>(OPT_ADAM);
   m.attr("OPT_ADAMW") = static_cast<int>(OPT_ADAMW);

@@ -750,6 +750,12 @@ void BucketSet::reduce_scatter(int g, bool pack) {
   p.status = cuda ? status_word_device() : status_word_host();
   p.timeout_ns = comm_->timeout_ns();
   p.amp = amp_.defined() ? reinterpret_cast<AmpState*>(amp_.data_ptr()) : nullptr;
+  if (clip_.defined()) {
+    DEAR_CHECK(static_cast<uint32_t>(b.rs_grid) <= kClipMaxCtas,
+               "norm_clip: reduce-scatter grid " << b.rs_grid << " exceeds " << kClipMaxCtas << " CTAs");
+    p.clip = reinterpret_cast<ClipState*>(clip_.data_ptr());
+    p.clip_slot = clip_slot_.at(g);
+  }
   if (b.rs_algo == RS_ALGO_PIPE) {
     // stripe-pipelined variant: stripe-major work list instead of the segment table (device kernel and host emulation)
     p.nstripes = b.nstripes;
@@ -797,6 +803,29 @@ void BucketSet::set_amp(std::optional<torch::Tensor> state) {
   amp_ = t;
 }
 
+void BucketSet::set_clip(std::optional<torch::Tensor> state, const std::vector<int64_t>& slots) {
+  if (!state.has_value() || !state->defined()) {
+    clip_ = torch::Tensor();
+    clip_slot_.clear();
+    return;
+  }
+  const torch::Tensor& t = *state;
+  DEAR_CHECK(slots.size() == buckets_.size(), "set_clip: one slot per bucket needed, got " << slots.size());
+  const int64_t nslots = (t.numel() - static_cast<int64_t>(sizeof(ClipState) / 4)) / (1 + static_cast<int64_t>(kClipMaxCtas));
+  DEAR_CHECK(t.scalar_type() == torch::kFloat && t.is_contiguous() && nslots >= 1 &&
+                 t.numel() == static_cast<int64_t>(clip_state_floats(static_cast<uint32_t>(nslots))),
+             "set_clip: the clipping state must be a contiguous float32 tensor of clip_state_floats(nslots) elements");
+  DEAR_CHECK(t.is_cuda() == comm_->is_cuda() && (!t.is_cuda() || t.device().index() == comm_->options().device),
+             "set_clip: the clipping state lives on the wrong device");
+  std::vector<uint32_t> s;
+  for (int64_t v : slots) {
+    DEAR_CHECK(v >= 0 && v < nslots, "set_clip: slot " << v << " out of range [0, " << nslots << ")");
+    s.push_back(static_cast<uint32_t>(v));
+  }
+  clip_ = t;
+  clip_slot_ = std::move(s);
+}
+
 void BucketSet::join(BucketSet& other) {
   if (!comm_->is_cuda() || &other == this) return;
   for (void* st : {other.stream_, other.ag_stream_}) {
@@ -806,7 +835,7 @@ void BucketSet::join(BucketSet& other) {
 }
 
 void BucketSet::allgather_update(int g, bool do_update, bool first_step, bool entry_barrier, bool zero_grad,
-                                 bool amp_decide) {
+                                 bool decide) {
   auto& b = buckets_.at(g);
   const bool cuda = comm_->is_cuda();
   AGParams p;
@@ -837,9 +866,10 @@ void BucketSet::allgather_update(int g, bool do_update, bool first_step, bool en
   p.first_step = first_step ? 1u : 0u;
   p.entry_barrier = entry_barrier ? 1u : 0u;
   p.amp = amp_.defined() ? reinterpret_cast<AmpState*>(amp_.data_ptr()) : nullptr;
-  DEAR_CHECK(!amp_decide || (p.amp != nullptr && entry_barrier && do_update),
-             "the deciding update of a scaled step needs a scaler state, the entry rendezvous and an update");
-  p.amp_decide = amp_decide ? 1u : 0u;
+  p.clip = clip_.defined() ? reinterpret_cast<ClipState*>(clip_.data_ptr()) : nullptr;
+  DEAR_CHECK(!decide || ((p.amp != nullptr || p.clip != nullptr) && entry_barrier && do_update),
+             "the deciding update of a step needs a scaler or clipping state, the entry rendezvous and an update");
+  p.decide = decide ? 1u : 0u;
   p.do_update = do_update ? 1u : 0u;
   p.sig = arena_->sig_table();
   p.ctrl = arena_->ctrl();

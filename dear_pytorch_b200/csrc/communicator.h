@@ -148,9 +148,13 @@ class BucketSet {
   std::string rs_plan(int g) const;
   // the pipelined kernel's work list of bucket g as rows (src, dst_off, nbytes, stripe, flags) — for tests / debugging
   std::vector<std::vector<int64_t>> pack_pieces(int g) const;
-  void allgather_update(int g, bool do_update, bool first_step, bool entry_barrier, bool zero_grad, bool amp_decide = false);
+  // `decide`: the step's deciding update (a scaler's skip decision, the clipping coefficient); needs the entry rendezvous
+  void allgather_update(int g, bool do_update, bool first_step, bool entry_barrier, bool zero_grad, bool decide = false);
   // Dynamic loss scaling: `state` is the engine's AmpState (int32[9], on this set's device), or None for the static path.
   void set_amp(std::optional<torch::Tensor> state);
+  // Global-norm clipping: `state` is the engine's ClipState (float32, clip_state_floats(nslots) elements, on this set's
+  // device) and `slots[g]` the engine-wide slot of local bucket g; None switches clipping off.
+  void set_clip(std::optional<torch::Tensor> state, const std::vector<int64_t>& slots);
   // The next update kernel on this set's all-gather stream waits for everything queued so far on both streams of
   // `other` (one decision per step across the sets of an engine).
   void join(BucketSet& other);
@@ -216,6 +220,8 @@ class BucketSet {
   void* upload_stream_ = nullptr;   // private non-capturing stream for tables built during a capture
   float grad_scale_ = 1.0f;
   torch::Tensor amp_;               // AmpState of the engine's dynamic loss scaler (undefined: static path)
+  torch::Tensor clip_;              // ClipState of the engine's global-norm clipping (undefined: no clipping)
+  std::vector<uint32_t> clip_slot_; // engine-wide slot of each local bucket
   void* ev_join_ = nullptr;
 };
 

@@ -106,10 +106,13 @@ constexpr uint32_t HYPER_SKIP = 2u;
 // torch-1.8 SGD semantics (reference dear/dear_dopt.py:310-336):
 //   g <- g + wd*p ; buf <- (first ? g : m*buf + (1-damp)*g) ; g <- nesterov ? g + m*buf : buf
 //   p <- p - lr*g
-// `g` is already averaged (the 1/P scale is fused into the reduce-scatter).
+// `g` is already averaged (the 1/P scale is fused into the reduce-scatter).  `coef` is the global-norm clipping
+// coefficient (1 without clipping); it is applied after the HYPER_SKIP test, so a parameter without a gradient on any
+// rank stays untouched even when `coef` is not finite.
 DEAR_HD float sgd_update(float p, float g, float& mom, const HyperSeg& h, bool first_step,
-                         bool has_mom_buf) {
+                         bool has_mom_buf, float coef) {
   if ((h.nesterov & HYPER_SKIP) && g == 0.f) return p;
+  g = g * coef;
   if (h.weight_decay != 0.f) g = g + h.weight_decay * p;
   if (h.momentum > 0.f && has_mom_buf) {
     float buf = first_step ? g : (h.momentum * mom + (1.f - h.dampening) * g);
@@ -122,8 +125,10 @@ DEAR_HD float sgd_update(float p, float g, float& mom, const HyperSeg& h, bool f
 // torch.optim.Adam / AdamW semantics (non-amsgrad): exp_avg `m`, exp_avg_sq `v`, bias corrections
 // bc1 = 1 - beta1^t, bc2 = 1 - beta2^t.  This extends the reference, whose DeAR path is SGD-only
 // (dear/dear_dopt.py:310-336; its BERT driver had to drop AdamW, dear/bert_benchmark.py:118-122).
-DEAR_HD float adam_update(float p, float g, float& m, float& v, const HyperSeg& h, float bc1, float sqrt_bc2) {
+DEAR_HD float adam_update(float p, float g, float& m, float& v, const HyperSeg& h, float bc1, float sqrt_bc2,
+                          float coef) {
   if ((h.nesterov & HYPER_SKIP) && g == 0.f) return p;
+  g = g * coef;                                    // clipping coefficient, as in sgd_update
   if (h.opt == OPT_ADAM && h.weight_decay != 0.f) g = g + h.weight_decay * p;
   m = h.momentum * m + (1.f - h.momentum) * g;
   v = h.beta2 * v + (1.f - h.beta2) * g * g;
@@ -192,6 +197,43 @@ DEAR_HD void amp_update_scale(AmpState* a, bool found_inf) {
   }
 }
 
+// ---- global gradient-norm clipping ----------------------------------------------
+//
+// Device-resident state of `norm_clip` (torch.nn.utils.clip_grad_norm_ semantics), one per engine, shared by every
+// BucketSet.  Buckets are numbered engine-wide ("slots").  Kernel A adds the square of every fp32 value it writes into
+// a per-thread sum, reduces it over the CTA, stores the CTA's partial, and the last CTA of the bucket sums the
+// partials in CTA order into the bucket's slot.  The step's deciding Kernel B sums the slots in slot order (this rank's
+// partial), exchanges partials at its entry rendezvous, and every CTA of every rank sums them in rank order, so all
+// ranks form the same `total_norm` and `coef` bit for bit.  The header is followed by float slot[nslots] and
+// float cta[nslots][kClipMaxCtas].
+constexpr uint32_t kClipMaxCtas = 1024;   // per-CTA partials per slot: Kernel A's grid may not exceed this with clipping
+struct ClipState {
+  float max_norm;
+  float total_norm;         // 2-norm of the step's averaged (unscaled) gradient, before clipping
+  float coef;               // min(1, max_norm / (total_norm + 1e-6)); NaN stays NaN, as in torch
+  uint32_t nslots;
+};
+
+DEAR_HD float* clip_slots(ClipState* c) { return reinterpret_cast<float*>(c + 1); }
+DEAR_HD float* clip_cta_partials(ClipState* c, uint32_t slot) {
+  return clip_slots(c) + c->nslots + size_t(slot) * kClipMaxCtas;
+}
+DEAR_HD size_t clip_state_floats(uint32_t nslots) { return sizeof(ClipState) / 4 + size_t(nslots) * (1 + kClipMaxCtas); }
+
+// torch: clip_coef = max_norm / (total_norm + 1e-6); clamp(max=1).  A comparison, not fminf: a NaN norm gives a NaN
+// coefficient, like torch.clamp.
+DEAR_HD float clip_coef(float max_norm, float total_norm) {
+  const float c = max_norm / (total_norm + 1e-6f);
+  return c > 1.f ? 1.f : c;
+}
+
+// The deciding kernel's partial sum of squares travels to every peer in a general channel of the bucket arena,
+// written before the AG_ARRIVE release store and read after its acquire.  Two channels by epoch parity: a rank can
+// write step s+1's partial while a peer still reads step s's (it cannot get to step s+2 before every peer arrived at
+// step s+1, which follows that peer's step-s decision on its all-gather stream).
+constexpr uint32_t CH_CLIP_PARTIAL = 12;   // and 13
+DEAR_HD uint32_t clip_channel(uint32_t epoch) { return CH_CLIP_PARTIAL + (epoch & 1u); }
+
 // ---- kernel parameter blocks ------------------------------------------------
 
 // Kernel A: fused [pack local grads -> symmetric bucket] + cross-GPU ready
@@ -217,7 +259,7 @@ struct RSParams {
   // stripe-pipelined variant (rs_pipe.cu): the shard is cut into `nstripes` stripes of `stripe_bytes`
   // (a multiple of kPipePackPiece); stripe k of EVERY shard is packed and published before stripe k+1
   uint32_t nstripes;
-  uint32_t reserved;
+  uint32_t clip_slot;      // engine-wide bucket number: Kernel A's sum of squares goes to clip_slots(clip)[clip_slot]
   uint64_t stripe_bytes;
   // pack work list of the pipelined variant: `pieces` (device) holds <= kPipePackPiece-byte copies in stripe-major
   // order, stripe k owning entries [piece_first[k], piece_first[k+1])
@@ -226,6 +268,8 @@ struct RSParams {
   // dynamic loss scale (nullptr => static path): the output is additionally divided by amp->scale, and a non-finite
   // output value sets amp->overflow
   AmpState* amp;
+  // global-norm clipping (nullptr => no clipping): sum of squares of the written shard into the bucket's slot
+  ClipState* clip;
 };
 
 // RS_READY flag encoding shared by both reduce-scatter kernels: (epoch << 8) | stripes_published; the one-shot
@@ -269,10 +313,13 @@ struct AGParams {
   uint32_t* status;
   uint64_t timeout_ns;
   // dynamic loss scale (nullptr => static path): the update is skipped when amp->found_inf is set.  The deciding kernel
-  // (`amp_decide`, the engine's first update of the step, which has `entry_barrier`) carries amp->overflow in its
+  // (`decide`, the engine's first update of the step, which has `entry_barrier`) carries amp->overflow in its
   // AG_ARRIVE flag, ORs every rank's bit and writes the decision.
   AmpState* amp;
-  uint32_t amp_decide;
+  uint32_t decide;
+  // global-norm clipping (nullptr => none): the deciding kernel forms clip->total_norm and clip->coef from every rank's
+  // partial sum of squares; every update kernel of the step multiplies clip->coef into the gradient
+  ClipState* clip;
 };
 
 // AG_ARRIVE flag encoding: (epoch << 1) | overflow bit of the sender (0 unless it is the deciding kernel).

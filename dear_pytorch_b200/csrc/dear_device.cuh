@@ -155,6 +155,39 @@ __device__ __forceinline__ bool all_finite(const float* f) {
   return ok;
 }
 
+// sum of squares of f[0..N) (global-norm clipping)
+template <int N>
+__device__ __forceinline__ float sum_sq(const float* f) {
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < N; ++i) s += f[i] * f[i];
+  return s;
+}
+
+// Clipping epilogue of Kernel A, called by the whole CTA before the grid-wide exit arrive: reduce the threads' sums of
+// squares in a fixed order (butterfly within each warp, then the warps in index order) and store the CTA's partial.
+// The same data-to-thread assignment therefore gives the same bits on every run.
+__device__ __forceinline__ void clip_store_cta_partial(ClipState* clip, uint32_t slot, float ss) {
+  __shared__ float s_warp[32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = ss;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (uint32_t w = 0; w < (blockDim.x >> 5); ++w) t += s_warp[w];
+    clip_cta_partials(clip, slot)[blockIdx.x] = t;
+  }
+}
+
+// Run by thread 0 of the last CTA to arrive: the bucket's slot = its CTAs' partials summed in CTA order.
+__device__ __forceinline__ void clip_combine_slot(ClipState* clip, uint32_t slot) {
+  const volatile float* part = clip_cta_partials(clip, slot);
+  float t = 0.f;
+  for (uint32_t b = 0; b < gridDim.x; ++b) t += part[b];
+  clip_slots(clip)[slot] = t;
+}
+
 // ----------------------------------------------------------------------------
 // element helpers
 // ----------------------------------------------------------------------------

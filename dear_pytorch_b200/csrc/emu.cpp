@@ -71,9 +71,11 @@ void rs_impl(const RSParams& p) {
   // 1/P (and 1/S of a static loss scale), times 1/scale of a dynamic one; a non-finite output sets amp->overflow
   const float scale = p.amp ? p.scale * (1.f / p.amp->scale) : p.scale;
   bool bad = false;
+  float ss = 0.f;                                // clipping: sum of squares of the written shard, in element order
   auto put = [&](uint64_t i, float v) {
     p.out[i] = v;
     if (p.amp && !std::isfinite(v)) bad = true;
+    if (p.clip) ss += v * v;
   };
   if (p.nstripes >= 1 && p.stripe_bytes > 0 && (p.pieces != nullptr || p.nstripes > 1)) {
     // stripe-pipelined variant (rs_pipe.cu): stripe k of every shard is packed from the stripe-major work list and
@@ -101,6 +103,7 @@ void rs_impl(const RSParams& p) {
       }
     }
     if (bad) __atomic_fetch_or(&p.amp->overflow, 1u, __ATOMIC_RELAXED);
+    if (p.clip) clip_slots(p.clip)[p.clip_slot] = ss;
     signal_all(p.sig, ch_done, p.rank, p.world, e);
     *epoch_p = e;
     return;
@@ -135,6 +138,7 @@ void rs_impl(const RSParams& p) {
     put(i, acc * scale);
   }
   if (bad) __atomic_fetch_or(&p.amp->overflow, 1u, __ATOMIC_RELAXED);
+  if (p.clip) clip_slots(p.clip)[p.clip_slot] = ss;
   signal_all(p.sig, ch_done, p.rank, p.world, e);
   *epoch_p = e;
 }
@@ -147,12 +151,34 @@ void ag_impl(const AGParams& p) {
   uint32_t* epoch_p = p.ctrl + ch_arrive;
   const uint32_t e = *epoch_p + 1;
   uint32_t found_inf = 0;
+  const bool clip = p.clip && p.do_update;
+  float coef = 1.f;
   if (p.entry_barrier) {
     // the deciding kernel's flags carry every rank's overflow bit (arrive_flag); OR them in rank order
-    const uint32_t ov = p.amp_decide ? p.amp->overflow : 0u;
+    const uint32_t ov = (p.decide && p.amp) ? p.amp->overflow : 0u;
+    if (clip && p.decide) {
+      // this rank's partial sum of squares (slot order) goes to every peer before the AG_ARRIVE release store
+      float t = 0.f;
+      for (uint32_t i = 0; i < p.clip->nslots; ++i) t += clip_slots(p.clip)[i];
+      uint32_t bits;
+      std::memcpy(&bits, &t, 4);
+      for (int r = 0; r < p.world; ++r) __atomic_store_n(flag_at(p.sig.ptr[r], clip_channel(e), p.rank), bits, __ATOMIC_RELAXED);
+    }
     signal_all(p.sig, ch_arrive, p.rank, p.world, arrive_flag(e, ov));
     wait_all(sig_local, ch_arrive, arrive_flag(e, 0), p.world, p.timeout_ns, p.status, ST_TIMEOUT_AG_ARRIVE);
-    if (p.amp_decide) {
+    if (clip && p.decide) {
+      float t = 0.f;
+      for (int r = 0; r < p.world; ++r) {
+        flag_load_acquire(flag_at(sig_local, ch_arrive, r));
+        const uint32_t bits = __atomic_load_n(flag_at(sig_local, clip_channel(e), r), __ATOMIC_RELAXED);
+        float f;
+        std::memcpy(&f, &bits, 4);
+        t += f;
+      }
+      p.clip->total_norm = std::sqrt(t);
+      p.clip->coef = clip_coef(p.clip->max_norm, p.clip->total_norm);
+    }
+    if (p.decide && p.amp) {
       for (int r = 0; r < p.world; ++r) found_inf |= flag_load_acquire(flag_at(sig_local, ch_arrive, r)) & 1u;
       p.amp->found_inf = found_inf;
       amp_update_scale(p.amp, found_inf != 0);
@@ -160,7 +186,8 @@ void ag_impl(const AGParams& p) {
       p.amp->overflow = 0;
     }
   }
-  if (p.amp && !p.amp_decide) found_inf = p.amp->found_inf;
+  if (p.amp && !p.decide) found_inf = p.amp->found_inf;
+  if (clip) coef = p.clip->coef;
   const bool upd = p.do_update && !found_inf;      // a skipped step is a pure all-gather of the unchanged shard
   const bool first_step = (p.amp && p.step_ctr) ? *p.step_ctr == 0 : p.first_step != 0;
   const uint64_t off = uint64_t(p.rank) * p.shard_elems;
@@ -174,10 +201,10 @@ void ag_impl(const AGParams& p) {
       if (adam) {
         const float bc1 = 1.f - std::pow(h.momentum, float(t_step));
         const float sqrt_bc2 = std::sqrt(1.f - std::pow(h.beta2, float(t_step)));
-        pv = adam_update(pv, p.grad_shard[i], p.mom_shard[i], p.var_shard[i], h, bc1, sqrt_bc2);
+        pv = adam_update(pv, p.grad_shard[i], p.mom_shard[i], p.var_shard[i], h, bc1, sqrt_bc2, coef);
       } else {
         float mv = (has_mom && !first_step) ? p.mom_shard[i] : 0.f;
-        pv = sgd_update(pv, p.grad_shard[i], mv, h, first_step, has_mom);
+        pv = sgd_update(pv, p.grad_shard[i], mv, h, first_step, has_mom, coef);
         if (has_mom && h.momentum > 0.f) p.mom_shard[i] = mv;
       }
       if (p.master_shard) p.master_shard[i] = pv;

@@ -41,7 +41,9 @@ constexpr int kPackVecPerThread = kPackTileBytes / 16 / kThreads;   // 8 x 128-b
 
 // AMP: dynamic loss scaling (p.amp != nullptr) — divide by the device-resident scale and test every written value for
 // finiteness.  A separate instantiation, so the static path compiles to exactly the work it did without a scaler.
-template <typename T, int W, bool MC, bool AMP>
+// CLIP: global-norm clipping (p.clip != nullptr) — add the square of every written value to a per-thread sum, which
+// the exit folds into the bucket's slot (clip_store_cta_partial / clip_combine_slot).  Also a separate instantiation.
+template <typename T, int W, bool MC, bool AMP, bool CLIP>
 __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
   using Tr = ElemTraits<T>;
   constexpr int EV = Tr::kPerVec;
@@ -63,6 +65,7 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
   // 1/P (and 1/S of a static loss scale), times 1/scale of a dynamic one
   const float scale = AMP ? p.scale * (1.f / *reinterpret_cast<volatile float*>(&p.amp->scale)) : p.scale;
   bool bad = false;                               // AMP: this thread wrote a non-finite value
+  float ss = 0.f;                                 // CLIP: sum of squares of the values this thread wrote
 
   // (0) my bucket may still be read by a peer's previous reduce-scatter.
   wait_all_peers(sig_local, ch_done, e - 1, world, p.timeout_ns, p.status, ST_TIMEOUT_RS_DONE);
@@ -107,6 +110,7 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
 #pragma unroll
             for (int x = 0; x < 8; ++x) f[x] *= scale;
             if (AMP) bad |= !all_finite<8>(f);
+            if (CLIP) ss += sum_sq<8>(f);
             float4* o4 = reinterpret_cast<float4*>(o + size_t(v) * 8);
             o4[0] = make_float4(f[0], f[1], f[2], f[3]);
             o4[1] = make_float4(f[EV - 4], f[EV - 3], f[EV - 2], f[EV - 1]);
@@ -115,6 +119,7 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
         for (uint32_t b = (nvec << 4) + tid * 2; b < nb; b += kThreads * 2) {
           const float x = zero ? 0.f : Tr::from_raw16(*reinterpret_cast<const uint16_t*>(s + b)) * scale;
           if (AMP) bad |= !isfinite(x);
+          if (CLIP) ss += x * x;
           o[b >> 1] = x;
         }
         continue;
@@ -145,6 +150,7 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
               float f[4] = {__uint_as_float(r[k].x) * scale, __uint_as_float(r[k].y) * scale,
                             __uint_as_float(r[k].z) * scale, __uint_as_float(r[k].w) * scale};
               if (AMP) bad |= !all_finite<4>(f);
+              if (CLIP) ss += sum_sq<4>(f);
               st_stream(d + (size_t(v) << 4),
                         make_uint4(__float_as_uint(f[0]), __float_as_uint(f[1]), __float_as_uint(f[2]), __float_as_uint(f[3])));
             }
@@ -152,6 +158,7 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
           for (uint32_t b = (nvec << 4) + tid * 4; b < nb; b += kThreads * 4) {
             const float x = *reinterpret_cast<const float*>(s + b) * scale;
             if (AMP) bad |= !isfinite(x);
+            if (CLIP) ss += x * x;
             *reinterpret_cast<float*>(d + b) = x;
           }
           continue;
@@ -200,6 +207,7 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
 #pragma unroll
             for (int k = 0; k < EV; ++k) f[k] *= scale;
             if (AMP) bad |= !all_finite<EV>(f);
+            if (CLIP) ss += sum_sq<EV>(f);
             float4* o = reinterpret_cast<float4*>(p.out + v * EV);
             o[0] = make_float4(f[0], f[1], f[2], f[3]);
             if (EV == 8) o[1] = make_float4(f[EV - 4], f[EV - 3], f[EV - 2], f[EV - 1]);
@@ -239,6 +247,7 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
 #pragma unroll
             for (int k = 0; k < EV; ++k) acc[k] *= scale;
             if (AMP) bad |= !all_finite<EV>(acc);
+            if (CLIP) ss += sum_sq<EV>(acc);
             float4* o = reinterpret_cast<float4*>(p.out + v * EV);
             o[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
             if (EV == 8) o[1] = make_float4(acc[EV - 4], acc[EV - 3], acc[EV - 2], acc[EV - 1]);
@@ -273,6 +282,7 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
 #pragma unroll
             for (int k = 0; k < EV; ++k) acc[u][k] *= scale;
             if (AMP) bad |= !all_finite<EV>(acc[u]);
+            if (CLIP) ss += sum_sq<EV>(acc[u]);
             float4* o = reinterpret_cast<float4*>(p.out + v * EV);
             o[0] = make_float4(acc[u][0], acc[u][1], acc[u][2], acc[u][3]);
             if (EV == 8) o[1] = make_float4(acc[u][EV - 4], acc[u][EV - 3], acc[u][EV - 2], acc[u][EV - 1]);
@@ -286,11 +296,13 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
   if (AMP) {
     if (__syncthreads_or(bad) && tid == 0) atomicOr(&p.amp->overflow, 1u);
   }
+  if (CLIP) clip_store_cta_partial(p.clip, p.clip_slot, ss);
 
   // (5) tell every peer I am done reading its bucket; advance the epoch.
   if (grid_arrive_is_last(cnt_exit)) {
     signal_all_peers(p.sig, ch_done, p.rank, world, e);
     if (tid == 0) {
+      if (CLIP) clip_combine_slot(p.clip, p.clip_slot);
       *cnt_exit = 0;
       *epoch_p = e;
     }
@@ -315,7 +327,9 @@ __device__ __forceinline__ void st_f32x(float* base, uint64_t v, int ev, const f
   if (ev == 8) m[1] = make_float4(in[4], in[5], in[6], in[7]);
 }
 
-template <typename T, int W, bool MC, bool ADAM>
+// CLIP: global-norm clipping (p.clip != nullptr): multiply the step's coefficient into the gradient.  A separate
+// instantiation, so the path without clipping compiles as before.
+template <typename T, int W, bool MC, bool ADAM, bool CLIP>
 __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
   using Tr = ElemTraits<T>;
   constexpr int EV = Tr::kPerVec;
@@ -342,14 +356,32 @@ __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
   // backward pass that still reads them: rendezvous at kernel entry.  With a dynamic loss scale the deciding kernel's
   // flags carry every rank's overflow bit: each CTA ORs them (fixed rank order), so all ranks reach the same decision.
   AmpState* const amp = p.amp;
+  ClipState* const clip = p.clip;
   uint32_t found_inf = 0;
+  float coef = 1.f;                               // CLIP: the step's clipping coefficient
   if (p.entry_barrier) {
     if (blockIdx.x == 0) {
-      const uint32_t ov = (p.amp_decide && tid < world) ? *reinterpret_cast<volatile uint32_t*>(&amp->overflow) : 0u;
+      // (with CLIP the deciding kernel may run without a scaler)
+      const bool amp_decide = p.decide && (!CLIP || amp != nullptr);
+      const uint32_t ov = (amp_decide && tid < world) ? *reinterpret_cast<volatile uint32_t*>(&amp->overflow) : 0u;
+      if (CLIP && p.decide) {
+        // this rank's partial: its slots in slot order.  Thread q stores it into peer q's pad and then, in
+        // signal_all_peers, fences and release-stores the AG_ARRIVE flag: a peer that acquires the flag sees the partial.
+        __shared__ float s_partial;
+        if (tid == 0) {
+          const volatile float* slots = clip_slots(clip);
+          float t = 0.f;
+          for (uint32_t i = 0; i < clip->nslots; ++i) t += slots[i];
+          s_partial = t;
+        }
+        __syncthreads();
+        if (tid < world)
+          *reinterpret_cast<volatile uint32_t*>(flag_at(p.sig.ptr[tid], clip_channel(e), p.rank)) = __float_as_uint(s_partial);
+      }
       signal_all_peers(p.sig, ch_arrive, p.rank, world, arrive_flag(e, ov));
     }
     wait_all_peers(sig_local, ch_arrive, arrive_flag(e, 0), world, p.timeout_ns, p.status, ST_TIMEOUT_AG_ARRIVE);
-    if (p.amp_decide) {
+    if (p.decide && (!CLIP || amp != nullptr)) {
       const uint32_t bit = tid < world ? (ld_acquire_sys(flag_at(sig_local, ch_arrive, tid)) & 1u) : 0u;
       found_inf = __syncthreads_or(bit) ? 1u : 0u;
       if (blockIdx.x == 0 && tid == 0) {
@@ -359,11 +391,32 @@ __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
         amp->overflow = 0;            // the next step's reduce-scatters are stream-ordered after this kernel
       }
     }
+    if (CLIP && p.decide) {
+      // every CTA of every rank sums the same W partials in rank order: one total and one coefficient everywhere
+      __shared__ float s_coef;
+      if (tid == 0) {
+        float t = 0.f;
+        for (int q = 0; q < world; ++q) {
+          const uint32_t* f = flag_at(sig_local, clip_channel(e), q);
+          (void)ld_acquire_sys(flag_at(sig_local, ch_arrive, q));
+          t += __uint_as_float(*reinterpret_cast<const volatile uint32_t*>(f));
+        }
+        const float total = sqrtf(t);
+        s_coef = clip_coef(clip->max_norm, total);
+        if (blockIdx.x == 0) {
+          clip->total_norm = total;
+          clip->coef = s_coef;
+        }
+      }
+      __syncthreads();
+      coef = s_coef;
+    }
   } else {
     __syncthreads();
   }
   // the step's other update kernels follow the deciding one on the all-gather stream(s)
-  if (amp != nullptr && !p.amp_decide) found_inf = *reinterpret_cast<volatile uint32_t*>(&amp->found_inf);
+  if (amp != nullptr && !p.decide) found_inf = *reinterpret_cast<volatile uint32_t*>(&amp->found_inf);
+  if (CLIP && !p.decide) coef = *reinterpret_cast<volatile float*>(&clip->coef);
   // a skipped step is a pure all-gather of the unchanged shard: same flag rounds, gradient bucket still zeroed
   const bool upd = p.do_update && !found_inf;
   // with a dynamic loss scale the host cannot know which update is the first one applied: count on the device
@@ -416,13 +469,14 @@ __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
               const float sqrt_bc2 = sqrtf(1.f - powf(h.beta2, float(t_step)));
 #pragma unroll
               for (int k = 0; k < EV; ++k)
-                pv[u][k] = adam_update(pv[u][k], gv[u][k], mv[u][k], vv[ADAM ? u : 0][k], h, bc1, sqrt_bc2);
+                pv[u][k] = adam_update(pv[u][k], gv[u][k], mv[u][k], vv[ADAM ? u : 0][k], h, bc1, sqrt_bc2,
+                                       CLIP ? coef : 1.f);
               st_f32x(p.mom_shard, v, EV, mv[u]);
               st_f32x(p.var_shard, v, EV, vv[ADAM ? u : 0]);
             } else {
 #pragma unroll
               for (int k = 0; k < EV; ++k)
-                pv[u][k] = sgd_update(pv[u][k], gv[u][k], mv[u][k], h, first_step, has_mom);
+                pv[u][k] = sgd_update(pv[u][k], gv[u][k], mv[u][k], h, first_step, has_mom, CLIP ? coef : 1.f);
               if (has_mom && h.momentum > 0.f) st_f32x(p.mom_shard, v, EV, mv[u]);
             }
             if (p.master_shard != nullptr) st_f32x(p.master_shard, v, EV, pv[u]);
@@ -626,21 +680,22 @@ static void check_launch(const char* what) {
     throw std::runtime_error(std::string("dear: launch of ") + what + " failed: " + cudaGetErrorString(err));
 }
 
-template <typename T, bool MC, bool AMP>
+template <typename T, bool MC, bool AMP, bool CLIP>
 static void launch_rs_wa(const RSParams& p, int grid, cudaStream_t s) {
   switch (p.world) {
-    case 1: rs_kernel<T, 1, MC, AMP><<<grid, kThreads, 0, s>>>(p); break;
-    case 2: rs_kernel<T, 2, MC, AMP><<<grid, kThreads, 0, s>>>(p); break;
-    case 4: rs_kernel<T, 4, MC, AMP><<<grid, kThreads, 0, s>>>(p); break;
-    case 8: rs_kernel<T, 8, MC, AMP><<<grid, kThreads, 0, s>>>(p); break;
-    default: rs_kernel<T, 0, MC, AMP><<<grid, kThreads, 0, s>>>(p); break;
+    case 1: rs_kernel<T, 1, MC, AMP, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    case 2: rs_kernel<T, 2, MC, AMP, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    case 4: rs_kernel<T, 4, MC, AMP, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    case 8: rs_kernel<T, 8, MC, AMP, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    default: rs_kernel<T, 0, MC, AMP, CLIP><<<grid, kThreads, 0, s>>>(p); break;
   }
 }
 
 template <typename T, bool MC>
 static void launch_rs_w(const RSParams& p, int grid, cudaStream_t s) {
-  if (p.amp != nullptr) launch_rs_wa<T, MC, true>(p, grid, s);
-  else launch_rs_wa<T, MC, false>(p, grid, s);
+  const bool clip = p.clip != nullptr;
+  if (p.amp != nullptr) clip ? launch_rs_wa<T, MC, true, true>(p, grid, s) : launch_rs_wa<T, MC, true, false>(p, grid, s);
+  else clip ? launch_rs_wa<T, MC, false, true>(p, grid, s) : launch_rs_wa<T, MC, false, false>(p, grid, s);
 }
 
 void launch_rs(const RSParams& p, int grid, cudaStream_t s) {
@@ -654,21 +709,22 @@ void launch_rs(const RSParams& p, int grid, cudaStream_t s) {
   check_launch("rs_kernel");
 }
 
-template <typename T, bool MC, bool ADAM>
+template <typename T, bool MC, bool ADAM, bool CLIP>
 static void launch_ag_wa(const AGParams& p, int grid, cudaStream_t s) {
   switch (p.world) {
-    case 1: ag_kernel<T, 1, MC, ADAM><<<grid, kThreads, 0, s>>>(p); break;
-    case 2: ag_kernel<T, 2, MC, ADAM><<<grid, kThreads, 0, s>>>(p); break;
-    case 4: ag_kernel<T, 4, MC, ADAM><<<grid, kThreads, 0, s>>>(p); break;
-    case 8: ag_kernel<T, 8, MC, ADAM><<<grid, kThreads, 0, s>>>(p); break;
-    default: ag_kernel<T, 0, MC, ADAM><<<grid, kThreads, 0, s>>>(p); break;
+    case 1: ag_kernel<T, 1, MC, ADAM, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    case 2: ag_kernel<T, 2, MC, ADAM, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    case 4: ag_kernel<T, 4, MC, ADAM, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    case 8: ag_kernel<T, 8, MC, ADAM, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    default: ag_kernel<T, 0, MC, ADAM, CLIP><<<grid, kThreads, 0, s>>>(p); break;
   }
 }
 
 template <typename T, bool MC>
 static void launch_ag_w(const AGParams& p, int grid, cudaStream_t s) {
-  if (p.adam && p.do_update) launch_ag_wa<T, MC, true>(p, grid, s);
-  else launch_ag_wa<T, MC, false>(p, grid, s);
+  const bool adam = p.adam && p.do_update, clip = p.clip != nullptr && p.do_update;
+  if (adam) clip ? launch_ag_wa<T, MC, true, true>(p, grid, s) : launch_ag_wa<T, MC, true, false>(p, grid, s);
+  else clip ? launch_ag_wa<T, MC, false, true>(p, grid, s) : launch_ag_wa<T, MC, false, false>(p, grid, s);
 }
 
 void launch_ag(const AGParams& p, int grid, cudaStream_t s) {

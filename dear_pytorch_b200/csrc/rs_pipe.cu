@@ -114,8 +114,8 @@ __device__ __forceinline__ uint32_t first_chunk(uint32_t k, uint64_t stripe_byte
   return (blockIdx.x + gridDim.x - before) % gridDim.x;
 }
 
-// AMP: dynamic loss scaling (p.amp != nullptr), see rs_kernel in kernels.cu.
-template <typename T, bool AMP>
+// AMP: dynamic loss scaling (p.amp != nullptr), CLIP: global-norm clipping (p.clip != nullptr), see rs_kernel in kernels.cu.
+template <typename T, bool AMP, bool CLIP>
 __global__ void __launch_bounds__(kPipeThreads, 1) rs_pipe_kernel(const RSParams p) {
   using Tr = ElemTraits<T>;
   constexpr int EV = Tr::kPerVec;
@@ -156,6 +156,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) rs_pipe_kernel(const RSParams
   const uint64_t cs = p.stripe_bytes;
   const uint64_t my_shard_off = uint64_t(p.rank) * SB;
   bool bad = false;                               // AMP: this thread wrote a non-finite value
+  float ss = 0.f;                                 // CLIP: sum of squares of the values this thread wrote
 
   if (tid >= 32 + kReduceThreads) {
     // ================================ PACK ================================
@@ -270,6 +271,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) rs_pipe_kernel(const RSParams
 #pragma unroll
             for (int x = 0; x < EV; ++x) acc[i][x] *= scale;
             if (AMP) bad |= !all_finite<EV>(acc[i]);
+            if (CLIP) ss += sum_sq<EV>(acc[i]);
             float4* o = reinterpret_cast<float4*>(out + size_t(v) * EV);
             o[0] = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
             if (EV == 8) o[1] = make_float4(acc[i][EV - 4], acc[i][EV - 3], acc[i][EV - 2], acc[i][EV - 1]);
@@ -283,11 +285,13 @@ __global__ void __launch_bounds__(kPipeThreads, 1) rs_pipe_kernel(const RSParams
   if (AMP) {
     if (__syncthreads_or(bad) && tid == 0) atomicOr(&p.amp->overflow, 1u);
   }
+  if (CLIP) clip_store_cta_partial(p.clip, p.clip_slot, ss);
 
   // (end) tell every peer I am done reading its bucket; advance the epoch.
   if (grid_arrive_is_last(cnt_exit)) {
     signal_all_peers(p.sig, ch_done, p.rank, world, e);
     if (tid == 0) {
+      if (CLIP) clip_combine_slot(p.clip, p.clip_slot);
       *cnt_exit = 0;
       *cnt_pack = 0;
       *epoch_p = e;
@@ -295,24 +299,25 @@ __global__ void __launch_bounds__(kPipeThreads, 1) rs_pipe_kernel(const RSParams
   }
 }
 
-static bool g_pipe_attr_set[6] = {false, false, false, false, false, false};
+static bool g_pipe_attr_set[12] = {false};
 
-template <typename T, bool AMP>
+template <typename T, bool AMP, bool CLIP>
 static void launch_pipe_ta(const RSParams& p, int grid, cudaStream_t s, int slot) {
   constexpr int smem = kPipeStages * kPipeChunk;
   if (!g_pipe_attr_set[slot]) {
-    cudaError_t err = cudaFuncSetAttribute(rs_pipe_kernel<T, AMP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t err = cudaFuncSetAttribute(rs_pipe_kernel<T, AMP, CLIP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (err != cudaSuccess)
       throw std::runtime_error(std::string("dear: cannot reserve shared memory for rs_pipe_kernel: ") + cudaGetErrorString(err));
     g_pipe_attr_set[slot] = true;
   }
-  rs_pipe_kernel<T, AMP><<<grid, kPipeThreads, smem, s>>>(p);
+  rs_pipe_kernel<T, AMP, CLIP><<<grid, kPipeThreads, smem, s>>>(p);
 }
 
 template <typename T>
 static void launch_pipe_t(const RSParams& p, int grid, cudaStream_t s, int slot) {
-  if (p.amp != nullptr) launch_pipe_ta<T, true>(p, grid, s, 3 + slot);
-  else launch_pipe_ta<T, false>(p, grid, s, slot);
+  const bool clip = p.clip != nullptr;
+  if (p.amp != nullptr) clip ? launch_pipe_ta<T, true, true>(p, grid, s, 9 + slot) : launch_pipe_ta<T, true, false>(p, grid, s, 3 + slot);
+  else clip ? launch_pipe_ta<T, false, true>(p, grid, s, 6 + slot) : launch_pipe_ta<T, false, false>(p, grid, s, slot);
 }
 
 void launch_rs_pipe(const RSParams& p, int grid, cudaStream_t s) {

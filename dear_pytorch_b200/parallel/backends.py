@@ -69,6 +69,7 @@ class _BackendBase:
         self.hyper: List[Optional[HyperSpec]] = [None] * nb
         self.grad_scale = 1.0
         self.amp: Optional[torch.Tensor] = None     # dynamic loss scaler state (parallel/grad_scaler.py), engine-owned
+        self.clip: Optional[torch.Tensor] = None    # global-norm clipping state (ClipState, csrc/dear_common.h), engine-owned
 
     # -- shard state ------------------------------------------------------------------
     def _alloc_shards(self):
@@ -117,6 +118,14 @@ class _BackendBase:
     def set_amp(self, state: Optional[torch.Tensor]) -> None:
         """Dynamic loss scaling: ``state`` is the engine's int32[9] AmpState (csrc/dear_common.h), or None."""
         self.amp = state
+
+    def clip_state_numel(self) -> int:
+        """float32 elements of the engine's clipping state (words 0-2: max_norm, total_norm, coef)."""
+        return 4
+
+    def set_clip(self, state: Optional[torch.Tensor]) -> None:
+        """Global-norm clipping: ``state`` is the engine's float32 ClipState, or None."""
+        self.clip = state
 
 
 # =====================================================================================
@@ -196,15 +205,25 @@ class NativeBackend(_BackendBase):
         for bs in self.sets.values():
             bs.set_amp(state)
 
+    def clip_state_numel(self):
+        return self.C.clip_state_floats(len(self.where))
+
+    def set_clip(self, state):
+        # slots are the engine-wide bucket indices: Kernel A of bucket g writes its sum of squares to slot g
+        self.clip = state
+        for bs in self.sets.values():
+            bs.set_clip(state, [g for g, (s, _) in enumerate(self.where) if s is bs])
+
     def allgather_update(self, g, do_update=True, first_step=False, zero_grad=False):
         bs, li = self.where[g]
         # the first bucket of every set carries the entry rendezvous: nobody overwrites a
         # peer's parameters before that peer has finished its backward pass.
         entry = self._first_in_set[id(bs)] == g
-        # dynamic loss scaling: bucket 0's update decides for the whole step.  With several dtype sets it waits for every
-        # set's reduce-scatters, and the other sets' first updates wait for it.
-        decide = self.amp is not None and g == 0 and do_update
-        if self.amp is not None and entry and len(self.sets) > 1:
+        # dynamic loss scaling and global-norm clipping: bucket 0's update decides for the whole step.  With several
+        # dtype sets it waits for every set's reduce-scatters, and the other sets' first updates wait for it.
+        deciding = self.amp is not None or self.clip is not None
+        decide = deciding and g == 0 and do_update
+        if deciding and entry and len(self.sets) > 1:
             for other in (self.sets.values() if decide else (self.where[0][0],)):
                 bs.join(other)
         bs.allgather_update(li, do_update, first_step, entry, zero_grad, decide)
@@ -294,6 +313,21 @@ class TorchBackend(_BackendBase):
             st[4] += 1
         self._overflow.zero_()
 
+    @torch.no_grad()
+    def _clip_decide(self):
+        """``torch.nn.utils.clip_grad_norm_`` over the averaged gradient: after the reduce-scatters every rank holds 1/P
+        of it exactly once, so the norm is one pass over the fp32 shards plus a one-element all-reduce.  The
+        coefficient is applied in the update (``_sgd_shard``).  Eager steps only."""
+        if self.cuda and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("norm_clip is not supported inside a CUDA-graph capture on the nccl backend")
+        shards = [s for s in self.grad_shard if s is not None]
+        sq = torch.stack(torch._foreach_norm(shards)).pow(2).sum().reshape(1)       # no shard-sized temporaries
+        if self.world > 1:
+            dist.all_reduce(sq, group=self.group)
+        total = sq.sqrt()
+        self.clip[1:2].copy_(total)
+        self.clip[2:3].copy_((self.clip[0:1] / (total + 1e-6)).clamp(max=1.0))
+
     def set_pack(self, g, src_ptrs, dst_off, nbytes, flags):
         pass    # gradients are accumulated straight into the bucket views
 
@@ -339,6 +373,8 @@ class TorchBackend(_BackendBase):
             sl = slice(a - lo, z - lo)
             p = master[sl] if master is not None else self._pbuf[g][a:z]
             d = self.grad_shard[g][sl]
+            if self.clip is not None:
+                d = d * self.clip[2]
             if opt != OPT_SGD:
                 t = self._t + 1
                 m, v = self.mom_shard[g][sl], self.var_shard[g][sl]
@@ -370,6 +406,8 @@ class TorchBackend(_BackendBase):
         with self._on_comm_stream():
             if do_update and g == 0 and self.amp is not None:
                 self._amp_decide()
+            if do_update and g == 0 and self.clip is not None:
+                self._clip_decide()
             if do_update:
                 self._sgd_shard(g, first_step)
             if self.master_shard[g] is not None:

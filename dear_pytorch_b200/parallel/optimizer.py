@@ -74,6 +74,8 @@ class DearEngine:
         self._mom_initialised = False
         self.num_updates = 0               # parameter updates applied so far (Adam bias correction)
         self.amp: Optional[torch.Tensor] = None   # dynamic loss scaler state (attach_scaler), survives re-bucketing
+        self._norm_clip: Optional[float] = None    # global-norm clipping (the norm_clip property)
+        self.clip: Optional[torch.Tensor] = None  # its device state (ClipState), rebuilt with the buckets
         self.flush_callbacks = []          # run by flush(): deferred work of the training loop (TrainStep.finish)
         if int(backward_passes_per_step) < 1:
             raise ValueError("backward_passes_per_step must be >= 1")
@@ -175,6 +177,8 @@ class DearEngine:
         be = self.backend
         be.set_grad_scale(1.0 / getattr(self, "loss_scale", 1.0))
         be.set_amp(self.amp)
+        self.clip = None
+        self._attach_clip()
         self.steal = be.steal_grads
         self._param_view: Dict[nn.Parameter, torch.Tensor] = {}
         self._grad_view: Dict[nn.Parameter, torch.Tensor] = {}
@@ -407,27 +411,57 @@ class DearEngine:
         ``optimizer.step(); scheduler.step()`` would have."""
         self._frozen_hyper = self._hyper_key_live()
 
-    @torch.no_grad()
-    def _clip_reduced_gradients(self):
-        """Global-norm clipping of the AVERAGED gradients, ``torch.nn.utils.clip_grad_norm_`` semantics (the reference's
-        WFBP optimizer clips per tensor after its all-reduce, wfbp/dopt.py:855-862; its DeAR factory accepts ``norm_clip``
-        and ignores it).  After the reduce-scatters every rank holds 1/P of the averaged gradient exactly once, so the
-        norm is one pass over the fp32 shards plus a one-element all-reduce; the shards are scaled in place before the
-        update kernels read them.  Costs the overlap of the first updates with the last reduce-scatters (the norm needs
-        all of them), no host synchronisation.  Eager steps only."""
+    # ------------------------------------------------------------------ global-norm clipping
+    # Semantics of ``torch.nn.utils.clip_grad_norm_`` on the AVERAGED (and, with a scaler, unscaled) gradient (the
+    # reference's WFBP optimizer clips per tensor after its all-reduce, wfbp/dopt.py:855-862; its DeAR factory accepts
+    # ``norm_clip`` and ignores it).  On the fused backends Kernel A sums the squares of the reduced shard per bucket and
+    # the step's first update kernel agrees on the norm with every rank at its entry rendezvous; every update kernel
+    # multiplies the coefficient into the gradient.  No extra pass over memory, no host synchronisation, and it can be
+    # captured in a CUDA graph.  ClipState words (csrc/dear_common.h): 0 max_norm, 1 total_norm, 2 coef, 3 slots.
+    @property
+    def norm_clip(self) -> Optional[float]:
+        return self._norm_clip
+
+    @norm_clip.setter
+    def norm_clip(self, value: Optional[float]):
+        """Takes effect at the next step; the value is written to the device on the current stream (outside any CUDA
+        graph), after every queued update."""
+        if value is not None:
+            value = float(value)
+            if not value > 0:
+                raise ValueError("norm_clip must be positive")
+        was_on = self._norm_clip is not None
+        self._norm_clip = value
+        if getattr(self, "backend", None) is None:
+            return
+        self.synchronize(host=False)
+        if value is not None and was_on and self.clip is not None:
+            self.clip[0].fill_(value)
+        else:
+            self.clip = None
+            self._attach_clip()
+
+    def _attach_clip(self):
+        """(Re)allocate the device clipping state for the current buckets and hand it to the backend."""
         be = self.backend
-        if self.device.type == "cuda" and torch.cuda.is_current_stream_capturing():
-            raise RuntimeError("norm_clip is not supported inside a CUDA-graph capture (TrainStep(use_graph=True))")
-        from .collectives import allreduce_
-        be.wait_all()                                    # the current stream now follows every reduce-scatter
-        shards = [s for s in be.grad_shard if s is not None]
-        sq = torch.stack(torch._foreach_norm(shards)).pow(2).sum().reshape(1)       # no shard-sized temporaries
-        allreduce_(sq, average=False)
-        total = sq.sqrt()
-        coef = (float(self.norm_clip) / (total + 1e-6)).clamp(max=1.0)
-        for s in shards:
-            s.mul_(coef)
-        self.last_grad_norm = total                      # device tensor (before clipping), for logging
+        if self._norm_clip is None or self.exclude_reducescatter or self.exclude_allgather:
+            be.set_clip(None)
+            return
+        st = torch.zeros(be.clip_state_numel(), dtype=torch.float32, device=self.device)
+        st[0] = self._norm_clip
+        st.view(torch.int32)[3] = len(self.plan.buckets)
+        self.clip = st
+        be.set_clip(st)
+
+    @property
+    def last_grad_norm(self) -> Optional[torch.Tensor]:
+        """2-norm of the last step's averaged gradient before clipping: a fresh 0-dim fp32 tensor, ordered on the
+        current stream after that step's deciding update.  None without clipping."""
+        if self.clip is None:
+            return None
+        if self._pending and self._pending[0]:
+            self._wait_bucket(0)                         # bucket 0's update decides the step
+        return self.clip[1].clone()
 
     def unfreeze_hyper(self):
         self._frozen_hyper = None
@@ -547,8 +581,6 @@ class DearEngine:
             self._drain_rs(force=True)
         if not self.exclude_allgather:
             self._refresh_hyper()
-            if getattr(self, "norm_clip", None) is not None and not self.exclude_reducescatter:
-                self._clip_reduced_gradients()
             be.fence()
             first = not self._mom_initialised
             for g in range(nb):
@@ -805,7 +837,8 @@ def DistributedOptimizer(optimizer, model, compression=None, is_sparse=False, de
     (Horovod's name; not in the reference) accumulates gradients locally over k backward passes and
     reduce-scatters them during the k-th; call ``step()`` once per k passes.  ``norm_clip=c`` (accepted and ignored by the
     reference's DeAR factory) clips the global norm of the averaged gradient to ``c`` like
-    ``torch.nn.utils.clip_grad_norm_`` before the update (``DearEngine._clip_reduced_gradients``).
+    ``torch.nn.utils.clip_grad_norm_`` before the update, inside the fused kernels (``DearEngine.norm_clip``; the norm
+    before clipping is ``engine.last_grad_norm``).
     """
     if threshold in (None, 0) and num_nearby_layers is None:
         threshold = float(os.environ.get("DEAR_THRESHOLD_MB", THRESHOLD))
@@ -817,9 +850,7 @@ def DistributedOptimizer(optimizer, model, compression=None, is_sparse=False, de
               exclude_parts=exclude_parts, policy=policy, verbose=verbose,
               backward_passes_per_step=backward_passes_per_step)
     if norm_clip is not None:
-        if norm_clip <= 0:
-            raise ValueError("norm_clip must be positive")
-        opt._dear.norm_clip = float(norm_clip)      # global-norm clipping of the averaged gradients (eager steps)
+        opt._dear.norm_clip = norm_clip             # global-norm clipping of the averaged gradients
     if loss_scale is not None:
         opt.set_loss_scale(loss_scale)
     if bo_tuning:

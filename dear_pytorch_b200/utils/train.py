@@ -77,6 +77,7 @@ class TrainStep:
         self.eager_calls = 0               # how many times the Python step body ran (incl. the capture)
         self.overlap_update = overlap_update
         self._pending_update = False       # rotated mode: gradients reduced, update not yet applied
+        self._clip_at_capture = None       # the engine's clipping state when the graph was captured
         if overlap_update and self._engine is not None:
             self._engine.flush_callbacks.append(self.finish)
 
@@ -174,6 +175,7 @@ class TrainStep:
             # an LR scheduler keeps working on a replayed graph; the native runtime refuses to capture such an upload
             eng.refresh_hyper_outside_graph()
             eng.synchronize(host=True)
+            self._clip_at_capture = eng.clip        # the captured kernels hold this clipping state's address
         torch.cuda.synchronize(dev)
         self._log("capturing")
         self._graph = torch.cuda.CUDAGraph()
@@ -206,6 +208,9 @@ class TrainStep:
                 return self._eager_on_side_stream(batch)
             return self._capture(batch)
         eng = self._engine
+        if eng is not None and eng.clip is not self._clip_at_capture:
+            raise RuntimeError("norm_clip was switched on or off after the training step was captured in a CUDA graph; "
+                               "its value may change between calls, but set it (or None) before the first call")
         if eng is not None and eng.hyper_changed():
             eng.refresh_hyper_outside_graph()
         _tree_zip_apply(lambda s, t: s.copy_(t, non_blocking=True) if s.data_ptr() != t.data_ptr() else None,

@@ -51,14 +51,14 @@ def _bench(rank, world, port, root, mbs, iters, warmup, q):
                         bs.reduce_scatter(0, True)
                         bs.wait_rs(0)
                     else:
-                        kw = {"amp_decide": True} if amp_on else {}
+                        kw = {"decide": True} if amp_on else {}
                         bs.allgather_update(0, True, False, True, False, **kw)
                         bs.wait_bucket(0)
                 ev[1].record()
                 torch.cuda.synchronize()
                 times[kernel] = ev[0].elapsed_time(ev[1]) * 1e3 / iters
                 if kernel == "A":
-                    bs.allgather_update(0, True, False, True, False, **({"amp_decide": True} if amp_on else {}))
+                    bs.allgather_update(0, True, False, True, False, **({"decide": True} if amp_on else {}))
                     bs.wait_bucket(0)
                     torch.cuda.synchronize()
             rows.append(dict(root=root, world=world, rank=rank, mb=mb, scaler=amp_on, kernel_a_us=round(times["A"], 2),
