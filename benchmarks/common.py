@@ -52,6 +52,9 @@ def add_common_args(ap):
     ap.add_argument("--norm-clip", type=float, default=None,
                     help="dear, dear-bo, dear-notf: clip the global gradient norm to this value (clip_grad_norm_ semantics, "
                          "inside the fused kernels)")
+    ap.add_argument("--grad-comm-dtype", choices=["fp32", "bf16", "fp16"], default="fp32",
+                    help="dear, dear-bo, dear-notf: dtype in which fp32 gradients are sent to the reduce-scatter (rounded "
+                         "on every rank, summed in fp32)")
     # flags of the reference's baseline drivers (horovod/, bytescheduler/, pytorch-ddp/ imagenet_benchmark.py)
     ap.add_argument("--fp16-allreduce", action="store_true", default=False,
                     help="--method horovod: fused buffers travel as fp16 (hvd.Compression.fp16)")
@@ -96,15 +99,17 @@ def wrap_optimizer(method, args, model, optimizer, profile_fn=None):
     world = dear.size()
     if method == "single" or (world == 1 and not method.startswith("dear")):
         return model, optimizer
+    wire = {"fp32": None, "bf16": torch.bfloat16, "fp16": torch.float16}[getattr(args, "grad_comm_dtype", "fp32")]
     if method == "dear":
         return model, dear.DistributedOptimizer(optimizer, model, threshold=args.threshold, exclude_parts=args.exclude_parts,
-                                                norm_clip=args.norm_clip)
+                                                norm_clip=args.norm_clip, grad_comm_dtype=wire)
     if method == "dear-bo":
         return model, dear.DistributedOptimizer(optimizer, model, threshold=args.threshold, exclude_parts=args.exclude_parts,
-                                                bo_tuning=True, norm_clip=args.norm_clip)
+                                                bo_tuning=True, norm_clip=args.norm_clip, grad_comm_dtype=wire)
     if method == "dear-notf":
         return model, dear.DistributedOptimizer(optimizer, model, threshold=None, num_nearby_layers=1,
-                                                exclude_parts=args.exclude_parts, norm_clip=args.norm_clip)
+                                                exclude_parts=args.exclude_parts, norm_clip=args.norm_clip,
+                                                grad_comm_dtype=wire)
     if method == "dear-naive":
         return model, variants.NaiveDistributedOptimizer(optimizer, model, exclude_parts=args.exclude_parts)
     if method == "dear-wt":

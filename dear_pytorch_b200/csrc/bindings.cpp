@@ -101,8 +101,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("launches", &Communicator::launches);
 
   py::class_<BucketSet, std::shared_ptr<BucketSet>>(m, "BucketSet")
-      .def(py::init<std::shared_ptr<Communicator>, std::vector<int64_t>, int, bool>(), py::arg("comm"),
-           py::arg("padded_numels"), py::arg("dtype"), py::arg("with_grad_buckets") = true)
+      .def(py::init<std::shared_ptr<Communicator>, std::vector<int64_t>, int, bool, std::optional<int>>(), py::arg("comm"),
+           py::arg("padded_numels"), py::arg("dtype"), py::arg("with_grad_buckets") = true,
+           py::arg("grad_dtype") = py::none())
       .def("num_buckets", &BucketSet::num_buckets)
       .def("has_multicast", &BucketSet::has_multicast)
       .def("param_buffer", &BucketSet::param_buffer)

@@ -375,17 +375,21 @@ void Communicator::barrier() {
 // BucketSet
 // ===========================================================================
 BucketSet::BucketSet(std::shared_ptr<Communicator> comm, std::vector<int64_t> padded_numels, int dtype,
-                     bool with_grad_buckets)
-    : comm_(std::move(comm)), dtype_(dtype), with_grad_(with_grad_buckets) {
+                     bool with_grad_buckets, std::optional<int> grad_dtype)
+    : comm_(std::move(comm)), dtype_(dtype), gdtype_(grad_dtype.value_or(dtype)), with_grad_(with_grad_buckets) {
   const int world = comm_->size();
   const size_t es = dtype_size(dtype);
+  const size_t ges = dtype_size(gdtype_);        // gradient (wire) element size
+  DEAR_CHECK(gdtype_ == dtype_ || (dtype_ == DT_F32 && (gdtype_ == DT_BF16 || gdtype_ == DT_F16)),
+             "grad_dtype must equal dtype, or be bf16 / fp16 for an fp32 set");
+  DEAR_CHECK(!converting() || world > 1, "a converting gradient set needs more than one rank (one rank has no wire)");
   DEAR_CHECK(static_cast<int>(padded_numels.size()) * kChannelsPerBucket + kGeneralChannels <= kNumChannels,
              "too many buckets (" << static_cast<long long>(padded_numels.size()) << ")");
   size_t off = 0;
   for (int64_t n : padded_numels) {
     DEAR_CHECK(n > 0 && n % world == 0, "bucket size must be a positive multiple of the world size");
     const int64_t shard = n / world;
-    DEAR_CHECK((shard * es) % 16 == 0, "shard bytes must be a multiple of 16");
+    DEAR_CHECK((shard * es) % 16 == 0 && (shard * ges) % 16 == 0, "shard bytes must be a multiple of 16");
     Bucket b;
     b.padded = n;
     b.shard = shard;
@@ -393,7 +397,7 @@ BucketSet::BucketSet(std::shared_ptr<Communicator> comm, std::vector<int64_t> pa
     off += (n * es + 255) / 256 * 256;
     if (with_grad_) {
       b.grad_off = off;
-      off += (n * es + 255) / 256 * 256;
+      off += (n * ges + 255) / 256 * 256;
     }
     buckets_.push_back(std::move(b));
   }
@@ -402,14 +406,15 @@ BucketSet::BucketSet(std::shared_ptr<Communicator> comm, std::vector<int64_t> pa
   // ---- per-bucket reduce-scatter plan (north star: "picked per bucket size") -------------------------------
   const CommOptions& o = comm_->options();
   for (auto& b : buckets_) {
-    const int64_t bytes = b.padded * static_cast<int64_t>(es);
-    const int64_t shard_bytes = b.shard * static_cast<int64_t>(es);
+    const int64_t bytes = b.padded * static_cast<int64_t>(ges);
+    const int64_t shard_bytes = b.shard * static_cast<int64_t>(ges);
     int algo = o.rs_algo;
     if (algo < 0) algo = (world > 1 && bytes >= o.pipe_min_bytes) ? RS_ALGO_PIPE : RS_ALGO_ONESHOT;
     // (the host emulation runs one algorithm; a FORCED pipe plan is still built there so that the stripe-major work
     // list of set_pack can be tested without a GPU)
     if (world == 1 || (!comm_->is_cuda() && o.rs_algo != RS_ALGO_PIPE)) algo = RS_ALGO_ONESHOT;
     if (algo == RS_ALGO_NVLS && !arena_->has_multicast()) algo = RS_ALGO_ONESHOT;
+    if (algo == RS_ALGO_PIPE && converting()) algo = RS_ALGO_ONESHOT;   // the pipelined pack does not convert
     b.rs_algo = algo;
     if (algo == RS_ALGO_PIPE) {
       int64_t k = std::max<int64_t>(1, std::min<int64_t>(16, bytes / std::max<int64_t>(1, o.stripe_target_bytes)));
@@ -485,7 +490,7 @@ torch::Tensor BucketSet::param_buffer(int g) {
 torch::Tensor BucketSet::grad_buffer(int g) {
   DEAR_CHECK(with_grad_, "this BucketSet has no gradient buckets");
   auto& b = buckets_.at(g);
-  return wrap(arena_->local_data() + b.grad_off, b.padded, dtype_, comm_->is_cuda(), comm_->options().device, arena_);
+  return wrap(arena_->local_data() + b.grad_off, b.padded, gdtype_, comm_->is_cuda(), comm_->options().device, arena_);
 }
 
 void BucketSet::set_step(int g, int64_t t) {
@@ -599,7 +604,7 @@ bool BucketSet::set_pack(int g, const std::vector<int64_t>& src_ptrs, const std:
   auto& b = buckets_.at(g);
   const size_t n = src_ptrs.size();
   DEAR_CHECK(dst_off_bytes.size() == n && nbytes.size() == n && flags.size() == n, "set_pack: ragged arguments");
-  const size_t es = dtype_size(dtype_);
+  const size_t es = dtype_size(gdtype_);        // offsets and sizes count gradient-bucket bytes
   std::vector<PackSeg> segs;
   segs.reserve(n);
   uint32_t tiles = 0;
@@ -739,14 +744,15 @@ void BucketSet::reduce_scatter(int g, bool pack) {
     p.nseg = static_cast<uint32_t>(b.pack_host.size());
     p.ntiles = b.ntiles;
     // one GPU: the pack writes the fp32 shard directly (fp32: copy; bf16 / fp16: widening, CUDA kernel only)
-    p.direct_out = (comm_->size() == 1 && (dtype_ == DT_F32 || cuda) && !b.pack_inplace) ? 1u : 0u;
+    p.direct_out = (comm_->size() == 1 && (gdtype_ == DT_F32 || cuda) && !b.pack_inplace) ? 1u : 0u;
   }
   p.sig = arena_->sig_table();
   p.ctrl = arena_->ctrl();
   p.bucket = static_cast<uint32_t>(g);
   p.rank = comm_->rank();
   p.world = comm_->size();
-  p.dtype = dtype_;
+  p.dtype = gdtype_;
+  p.src_f32 = converting() ? 1u : 0u;
   p.status = cuda ? status_word_device() : status_word_host();
   p.timeout_ns = comm_->timeout_ns();
   p.amp = amp_.defined() ? reinterpret_cast<AmpState*>(amp_.data_ptr()) : nullptr;
@@ -860,7 +866,7 @@ void BucketSet::allgather_update(int g, bool do_update, bool first_step, bool en
   DEAR_CHECK(dtype_ == DT_F32 || p.master_shard != nullptr, "low-precision parameter buckets need an fp32 master shard");
   if (zero_grad && with_grad_) {
     p.zero_grad = arena_->local_data() + b.grad_off;
-    p.zero_bytes = static_cast<uint64_t>(b.padded) * dtype_size(dtype_);
+    p.zero_bytes = static_cast<uint64_t>(b.padded) * dtype_size(gdtype_);
   }
   p.shard_elems = static_cast<uint64_t>(b.shard);
   p.first_step = first_step ? 1u : 0u;
@@ -939,6 +945,7 @@ std::string BucketSet::rs_plan(int g) const {
   static const char* names[] = {"oneshot", "pipe", "nvls"};
   Msg o;
   o << names[b.rs_algo] << ":grid=" << b.rs_grid << ":stripes=" << b.nstripes << ":stripe_bytes=" << b.stripe_bytes;
+  if (converting()) o << ":wire=" << (gdtype_ == DT_BF16 ? "bf16" : "fp16");
   return o.str();
 }
 

@@ -120,14 +120,17 @@ class Communicator : public std::enable_shared_from_this<Communicator> {
 
 class BucketSet {
  public:
+  // `grad_dtype` (default: `dtype`) is the element type of the gradient buckets.  An fp32 set may send its gradients
+  // as bf16 / fp16: the pack rounds them, the pull accumulates in fp32 (a "converting" set, world > 1 only).
   BucketSet(std::shared_ptr<Communicator> comm, std::vector<int64_t> padded_numels, int dtype,
-            bool with_grad_buckets);
+            bool with_grad_buckets, std::optional<int> grad_dtype = std::nullopt);
   ~BucketSet();
 
   int num_buckets() const { return static_cast<int>(buckets_.size()); }
   torch::Tensor param_buffer(int g);
   torch::Tensor grad_buffer(int g);
   bool has_multicast() const { return arena_->has_multicast(); }
+  bool converting() const { return gdtype_ != dtype_; }
 
   void set_shards(int g, torch::Tensor grad_shard, std::optional<torch::Tensor> mom,
                   std::optional<torch::Tensor> master, std::optional<torch::Tensor> var);
@@ -212,6 +215,7 @@ class BucketSet {
   std::shared_ptr<SymmArena> arena_;
   std::vector<Bucket> buckets_;
   int dtype_;
+  int gdtype_;                  // gradient-bucket dtype (== dtype_ unless the set converts fp32 gradients)
   bool with_grad_;
   void* stream_ = nullptr;      // cudaStream_t (high priority): reduce-scatters, table uploads
   void* ag_stream_ = nullptr;   // cudaStream_t: update + all-gather kernels (== stream_ unless separate_ag_stream)

@@ -73,6 +73,8 @@ struct PeerTable {
 };
 
 // One gradient segment of a bucket (== one parameter's gradient).
+// In a converting set (fp32 parameters whose gradients travel as bf16 / fp16, RSParams::src_f32) `dst_off` and
+// `nbytes` count bucket (wire) bytes, and the pack reads the fp32 source at twice those offsets and byte counts.
 struct PackSeg {
   const void* src;        // local gradient storage; nullptr => nothing to copy
   uint64_t dst_off;       // byte offset inside the bucket
@@ -270,6 +272,9 @@ struct RSParams {
   AmpState* amp;
   // global-norm clipping (nullptr => no clipping): sum of squares of the written shard into the bucket's slot
   ClipState* clip;
+  // converting set: the gradients are fp32 and the pack rounds them to `dtype` (round to nearest even) on the way
+  // into the bucket; the pull is the ordinary 16-bit one.  Never set at world 1 (one rank has no wire).
+  uint32_t src_f32;
 };
 
 // RS_READY flag encoding shared by both reduce-scatter kernels: (epoch << 8) | stripes_published; the one-shot

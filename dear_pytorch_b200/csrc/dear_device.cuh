@@ -204,6 +204,7 @@ template <> struct ElemTraits<float> {
   }
   __device__ static uint4 mc_reduce(const void* mc) { return multimem_ld_reduce_f32(mc); }
   __device__ static float from_raw16(uint16_t) { return 0.f; }   // (not a 16-bit type)
+  __device__ static uint16_t to_raw16(float) { return 0; }
 };
 template <> struct ElemTraits<__nv_bfloat16> {
   static constexpr int kPerVec = 8;
@@ -226,6 +227,7 @@ template <> struct ElemTraits<__nv_bfloat16> {
   }
   __device__ static uint4 mc_reduce(const void* mc) { return multimem_ld_reduce_bf16(mc); }
   __device__ static float from_raw16(uint16_t r) { return __uint_as_float(uint32_t(r) << 16); }
+  __device__ static uint16_t to_raw16(float x) { return __bfloat16_as_ushort(__float2bfloat16_rn(x)); }
 };
 template <> struct ElemTraits<__half> {
   static constexpr int kPerVec = 8;
@@ -249,6 +251,7 @@ template <> struct ElemTraits<__half> {
   }
   __device__ static uint4 mc_reduce(const void* mc) { return multimem_ld_reduce_f16(mc); }
   __device__ static float from_raw16(uint16_t r) { return __half2float(__ushort_as_half(r)); }
+  __device__ static uint16_t to_raw16(float x) { return __half_as_ushort(__float2half_rn(x)); }
 };
 
 }  // namespace dear

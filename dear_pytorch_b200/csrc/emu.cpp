@@ -120,6 +120,12 @@ void rs_impl(const RSParams& p) {
       const uint32_t nb = left < kPackTileBytes ? uint32_t(left) : kPackTileBytes;
       if (sg.flags & SEG_ZERO_FILL) {
         std::memset(bucket + sg.dst_off + off2, 0, nb);
+      } else if (sg.src != nullptr && p.src_f32) {
+        // converting set: fp32 source at twice the bucket offsets, rounded to T (c10's round to nearest even, as
+        // torch's .to(): NaN stays NaN, fp16 overflow becomes inf)
+        const float* src = reinterpret_cast<const float*>(sg.src) + off2 / sizeof(T);
+        T* dst = reinterpret_cast<T*>(bucket + sg.dst_off + off2);
+        for (uint32_t k = 0; k < nb / sizeof(T); ++k) dst[k] = static_cast<T>(src[k]);
       } else if (sg.src != nullptr && direct) {
         // fp32, one rank: the pack writes the reduced shard, so it applies the factor the reduction would have
         const float* src = reinterpret_cast<const float*>(reinterpret_cast<const char*>(sg.src) + off2);

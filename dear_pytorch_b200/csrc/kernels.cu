@@ -43,7 +43,9 @@ constexpr int kPackVecPerThread = kPackTileBytes / 16 / kThreads;   // 8 x 128-b
 // finiteness.  A separate instantiation, so the static path compiles to exactly the work it did without a scaler.
 // CLIP: global-norm clipping (p.clip != nullptr) — add the square of every written value to a per-thread sum, which
 // the exit folds into the bucket's slot (clip_store_cta_partial / clip_combine_slot).  Also a separate instantiation.
-template <typename T, int W, bool MC, bool AMP, bool CLIP>
+// CVT: a converting set (p.src_f32) — the gradients are fp32 and the pack rounds them to the 16-bit T of the bucket;
+// the pull phase is the ordinary one of T.  Instantiated for W != 1 only.
+template <typename T, int W, bool MC, bool AMP, bool CLIP, bool CVT = false>
 __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
   using Tr = ElemTraits<T>;
   constexpr int EV = Tr::kPerVec;
@@ -133,6 +135,31 @@ __global__ void __launch_bounds__(kThreads, 1) rs_kernel(const RSParams p) {
         }
         for (uint32_t b = (nvec << 4) + tid * 2; b < nb; b += kThreads * 2)
           *reinterpret_cast<uint16_t*>(d + b) = 0;
+      } else if (CVT && sg.src != nullptr) {
+        // fp32 source, 16-bit bucket: a tile is kPackTileBytes of the bucket and twice that of the source.  Two 128-bit
+        // fp32 loads make one 128-bit store of 8 rounded elements (16 loads in flight per thread).
+        const char* s = reinterpret_cast<const char*>(sg.src) + 2 * off;
+        uint4 r[kPackVecPerThread][2];
+#pragma unroll
+        for (int k = 0; k < kPackVecPerThread; ++k) {
+          const uint32_t v = tid + k * kThreads;
+          if (v < nvec) {
+            r[k][0] = ld_stream(s + (size_t(v) << 5));
+            r[k][1] = ld_stream(s + (size_t(v) << 5) + 16);
+          }
+        }
+#pragma unroll
+        for (int k = 0; k < kPackVecPerThread; ++k) {
+          const uint32_t v = tid + k * kThreads;
+          if (v < nvec) {
+            float f[8];
+            ElemTraits<float>::unpack(r[k][0], f);
+            ElemTraits<float>::unpack(r[k][1], f + 4);
+            st_stream(d + (size_t(v) << 4), Tr::pack(f));
+          }
+        }
+        for (uint32_t b = (nvec << 4) + tid * 2; b < nb; b += kThreads * 2)
+          *reinterpret_cast<uint16_t*>(d + b) = Tr::to_raw16(*reinterpret_cast<const float*>(s + 2 * size_t(b)));
       } else if (sg.src != nullptr) {
         const char* s = reinterpret_cast<const char*>(sg.src) + off;
         uint4 r[kPackVecPerThread];
@@ -680,26 +707,40 @@ static void check_launch(const char* what) {
     throw std::runtime_error(std::string("dear: launch of ") + what + " failed: " + cudaGetErrorString(err));
 }
 
-template <typename T, bool MC, bool AMP, bool CLIP>
+template <typename T, bool MC, bool AMP, bool CLIP, bool CVT>
 static void launch_rs_wa(const RSParams& p, int grid, cudaStream_t s) {
   switch (p.world) {
-    case 1: rs_kernel<T, 1, MC, AMP, CLIP><<<grid, kThreads, 0, s>>>(p); break;
-    case 2: rs_kernel<T, 2, MC, AMP, CLIP><<<grid, kThreads, 0, s>>>(p); break;
-    case 4: rs_kernel<T, 4, MC, AMP, CLIP><<<grid, kThreads, 0, s>>>(p); break;
-    case 8: rs_kernel<T, 8, MC, AMP, CLIP><<<grid, kThreads, 0, s>>>(p); break;
-    default: rs_kernel<T, 0, MC, AMP, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    case 1:
+      if constexpr (CVT) throw std::runtime_error("dear: a converting gradient set needs more than one rank");
+      else rs_kernel<T, 1, MC, AMP, CLIP><<<grid, kThreads, 0, s>>>(p);
+      break;
+    case 2: rs_kernel<T, 2, MC, AMP, CLIP, CVT><<<grid, kThreads, 0, s>>>(p); break;
+    case 4: rs_kernel<T, 4, MC, AMP, CLIP, CVT><<<grid, kThreads, 0, s>>>(p); break;
+    case 8: rs_kernel<T, 8, MC, AMP, CLIP, CVT><<<grid, kThreads, 0, s>>>(p); break;
+    default: rs_kernel<T, 0, MC, AMP, CLIP, CVT><<<grid, kThreads, 0, s>>>(p); break;
   }
 }
 
-template <typename T, bool MC>
+template <typename T, bool MC, bool CVT = false>
 static void launch_rs_w(const RSParams& p, int grid, cudaStream_t s) {
   const bool clip = p.clip != nullptr;
-  if (p.amp != nullptr) clip ? launch_rs_wa<T, MC, true, true>(p, grid, s) : launch_rs_wa<T, MC, true, false>(p, grid, s);
-  else clip ? launch_rs_wa<T, MC, false, true>(p, grid, s) : launch_rs_wa<T, MC, false, false>(p, grid, s);
+  if (p.amp != nullptr) clip ? launch_rs_wa<T, MC, true, true, CVT>(p, grid, s) : launch_rs_wa<T, MC, true, false, CVT>(p, grid, s);
+  else clip ? launch_rs_wa<T, MC, false, true, CVT>(p, grid, s) : launch_rs_wa<T, MC, false, false, CVT>(p, grid, s);
 }
 
 void launch_rs(const RSParams& p, int grid, cudaStream_t s) {
   const bool mc = p.mc_grad != nullptr;
+  if (p.src_f32) {
+    switch (p.dtype) {
+      case DT_BF16:
+        mc ? launch_rs_w<__nv_bfloat16, true, true>(p, grid, s) : launch_rs_w<__nv_bfloat16, false, true>(p, grid, s);
+        break;
+      case DT_F16: mc ? launch_rs_w<__half, true, true>(p, grid, s) : launch_rs_w<__half, false, true>(p, grid, s); break;
+      default: throw std::runtime_error("dear: a converting gradient set sends bf16 or fp16");
+    }
+    check_launch("rs_kernel");
+    return;
+  }
   switch (p.dtype) {
     case DT_F32: mc ? launch_rs_w<float, true>(p, grid, s) : launch_rs_w<float, false>(p, grid, s); break;
     case DT_BF16: mc ? launch_rs_w<__nv_bfloat16, true>(p, grid, s) : launch_rs_w<__nv_bfloat16, false>(p, grid, s); break;

@@ -56,11 +56,14 @@ class HyperSpec:
 class _BackendBase:
     steal_grads = False
 
-    def __init__(self, plan: BucketPlan, rank: int, world: int, device: torch.device):
+    def __init__(self, plan: BucketPlan, rank: int, world: int, device: torch.device,
+                 grad_comm_dtype: Optional[torch.dtype] = None):
         self.plan = plan
         self.rank = rank
         self.world = world
         self.device = device
+        # fp32 gradients travel as this 16-bit dtype (DearEngine.grad_comm_dtype); one rank has no wire
+        self.wire = grad_comm_dtype if world > 1 else None
         nb = len(plan.buckets)
         self.grad_shard: List[torch.Tensor] = [None] * nb
         self.mom_shard: List[Optional[torch.Tensor]] = [None] * nb
@@ -134,8 +137,9 @@ class _BackendBase:
 class NativeBackend(_BackendBase):
     steal_grads = True
 
-    def __init__(self, comm, plan: BucketPlan, rank: int, world: int, device: torch.device):
-        super().__init__(plan, rank, world, device)
+    def __init__(self, comm, plan: BucketPlan, rank: int, world: int, device: torch.device,
+                 grad_comm_dtype: Optional[torch.dtype] = None):
+        super().__init__(plan, rank, world, device, grad_comm_dtype)
         C = ops.require_native()
         self.C = C
         self.comm = comm
@@ -148,7 +152,10 @@ class NativeBackend(_BackendBase):
         self.sets = {}
         self.where: List[Tuple[object, int]] = [None] * len(plan.buckets)
         for dt, idxs in by_dtype.items():
-            bs = C.BucketSet(comm, [plan.buckets[g].padded_numel for g in idxs], getattr(C, _DT_CODE[dt]), True)
+            # fp32 sets with a wire dtype are converting sets: 16-bit gradient buckets, the pack rounds
+            wire = self.wire if dt == torch.float32 and self.wire is not None else dt
+            bs = C.BucketSet(comm, [plan.buckets[g].padded_numel for g in idxs], getattr(C, _DT_CODE[dt]), True,
+                             getattr(C, _DT_CODE[wire]))
             self.sets[dt] = bs
             for li, g in enumerate(idxs):
                 self.where[g] = (bs, li)
@@ -262,8 +269,9 @@ class NativeBackend(_BackendBase):
 class TorchBackend(_BackendBase):
     steal_grads = False
 
-    def __init__(self, group, plan: BucketPlan, rank: int, world: int, device: torch.device):
-        super().__init__(plan, rank, world, device)
+    def __init__(self, group, plan: BucketPlan, rank: int, world: int, device: torch.device,
+                 grad_comm_dtype: Optional[torch.dtype] = None):
+        super().__init__(plan, rank, world, device, grad_comm_dtype)
         self.group = group
         self.cuda = device.type == "cuda"
         self._pbuf = [torch.zeros(b.padded_numel, dtype=b.dtype, device=device) for b in plan.buckets]
@@ -341,6 +349,10 @@ class TorchBackend(_BackendBase):
         if self.cuda:
             self.stream.wait_stream(torch.cuda.current_stream(self.device))
         with self._on_comm_stream():
+            if self.wire is not None and self._gbuf[g].dtype == torch.float32:
+                # the fused backends' rounding (grad_comm_dtype) before the same fp32 collective: same arithmetic up to
+                # the summation order, no bandwidth saved
+                self._gbuf[g].copy_(self._gbuf[g].to(self.wire))
             if self.world > 1:
                 dist.reduce_scatter_tensor(self._rs_out[g], self._gbuf[g], op=dist.ReduceOp.SUM, group=self.group)
             else:

@@ -56,7 +56,12 @@ class DearEngine:
 
     def __init__(self, optimizer: torch.optim.Optimizer, model: nn.Module, *, threshold=THRESHOLD,
                  num_nearby_layers=NUM_NEARBY_LAYERS, exclude_parts: str = "", policy=None, verbose=True,
-                 backward_passes_per_step: int = 1):
+                 backward_passes_per_step: int = 1, grad_comm_dtype: Optional[torch.dtype] = None):
+        if grad_comm_dtype not in (None, torch.float32, torch.bfloat16, torch.float16):
+            raise ValueError("grad_comm_dtype must be None, torch.float32, torch.bfloat16 or torch.float16; got %r"
+                             % (grad_comm_dtype,))
+        # fp32 gradients cross the wire as this 16-bit dtype (None: as fp32); fixed for the engine's lifetime
+        self._grad_comm_dtype = None if grad_comm_dtype in (None, torch.float32) else grad_comm_dtype
         if not runtime.is_initialized():
             runtime.init()
         self.opt = optimizer
@@ -163,11 +168,23 @@ class DearEngine:
         h0 = runtime.broadcast_object(h, src=0)
         if h != h0:
             raise RuntimeError("rank %d built a different bucket plan than rank 0 (models differ?)" % self.rank)
+        # ranks that disagree would pack gradients of different formats into each other's buckets: every rank learns
+        # every setting, so all of them raise
+        wires = [None] * self.world
+        torch.distributed.all_gather_object(wires, str(self._grad_comm_dtype), group=runtime.group())
+        if len(set(wires)) != 1:
+            raise RuntimeError("the ranks disagree on grad_comm_dtype: %s (rank order)" % ", ".join(wires))
+
+    @property
+    def grad_comm_dtype(self) -> Optional[torch.dtype]:
+        """16-bit dtype in which fp32 gradients are sent to the reduce-scatter (None: fp32, the default)."""
+        return self._grad_comm_dtype
 
     def _make_backend(self):
         if self.backend_name in ("b200", "emu"):
-            return NativeBackend(runtime.communicator(), self.plan, self.rank, self.world, self.device)
-        return TorchBackend(runtime.group(), self.plan, self.rank, self.world, self.device)
+            return NativeBackend(runtime.communicator(), self.plan, self.rank, self.world, self.device,
+                                 self._grad_comm_dtype)
+        return TorchBackend(runtime.group(), self.plan, self.rank, self.world, self.device, self._grad_comm_dtype)
 
     @torch.no_grad()
     def _build(self, initial: bool, carry: Optional[dict] = None):
@@ -199,8 +216,9 @@ class DearEngine:
                     p.grad = None
                 else:
                     p.grad = gv
-                # Linear weights: the wgrad GEMM writes its slice of the gradient bucket directly (ops/direct_wgrad.py)
-                if self._direct_wgrad and p.dim() == 2 and gv.is_contiguous():
+                # Linear weights: the wgrad GEMM writes its slice of the gradient bucket directly (ops/direct_wgrad.py).
+                # Not into a 16-bit bucket of fp32 gradients (grad_comm_dtype): those go through the converting pack.
+                if self._direct_wgrad and p.dim() == 2 and gv.is_contiguous() and gv.dtype == p.dtype:
                     p._dear_grad_view = gv
                     p._dear_grad_written = False
                     self._direct_params.append(p)
@@ -223,8 +241,10 @@ class DearEngine:
         self._inflight: Dict[int, List[torch.Tensor]] = {}
         self._src = [[0] * n for n in self._n_params]
         self._flags = [[0] * n for n in self._n_params]
-        self._dst_off = [[s.start * s.param.element_size() for s in b.slots] for b in plan.buckets]
-        self._nbytes = [[s.numel * s.param.element_size() for s in b.slots] for b in plan.buckets]
+        # pack tables count gradient-bucket bytes (2 per element when fp32 gradients travel at 16 bits)
+        es = [be.grad_buffer(b.index).element_size() for b in plan.buckets]
+        self._dst_off = [[s.start * es[b.index] for s in b.slots] for b in plan.buckets]
+        self._nbytes = [[s.numel * es[b.index] for s in b.slots] for b in plan.buckets]
         self._hyper_key = [None] * nb
         self._absent = [()] * nb           # per bucket: slots that received no gradient in the current step
         self._module_bucket = list(plan.module_bucket)
@@ -761,7 +781,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
     reference uses, dear/dear_dopt.py:395-398)."""
 
     def __init__(self, params, model, threshold=THRESHOLD, num_nearby_layers=NUM_NEARBY_LAYERS,
-                 exclude_parts="", policy=None, verbose=True, backward_passes_per_step=1):
+                 exclude_parts="", policy=None, verbose=True, backward_passes_per_step=1, grad_comm_dtype=None):
         super(self.__class__, self).__init__(params)
         if not isinstance(self, (torch.optim.SGD, torch.optim.Adam, torch.optim.AdamW)):
             raise TypeError(
@@ -776,7 +796,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                 raise ValueError("maximize=True is not supported")
         self._dear = DearEngine(self, model, threshold=threshold, num_nearby_layers=num_nearby_layers,
                                 exclude_parts=exclude_parts, policy=policy, verbose=verbose,
-                                backward_passes_per_step=backward_passes_per_step)
+                                backward_passes_per_step=backward_passes_per_step, grad_comm_dtype=grad_comm_dtype)
 
     # -- torch.optim.Optimizer API ---------------------------------------------------
     def step(self, closure=None):
@@ -825,7 +845,7 @@ def DistributedOptimizer(optimizer, model, compression=None, is_sparse=False, de
                          layerwise_times=None, norm_clip=None, threshold=None, writer=None, gradient_path=None,
                          fp16=False, mgwfbp=False, rdma=False, multi_job_scheduling=False, exclude_parts="",
                          num_nearby_layers=None, policy=None, verbose=True, bo_tuning=False, bo_kwargs=None,
-                         backward_passes_per_step=1, loss_scale=None):
+                         backward_passes_per_step=1, loss_scale=None, grad_comm_dtype=None):
     """Wrap ``optimizer`` (``torch.optim.SGD`` / ``Adam`` / ``AdamW``) for DeAR data-parallel training of ``model``.
 
     Signature-compatible with the reference factory (dear/dear_dopt.py:381-398): the Horovod-era
@@ -838,7 +858,11 @@ def DistributedOptimizer(optimizer, model, compression=None, is_sparse=False, de
     reduce-scatters them during the k-th; call ``step()`` once per k passes.  ``norm_clip=c`` (accepted and ignored by the
     reference's DeAR factory) clips the global norm of the averaged gradient to ``c`` like
     ``torch.nn.utils.clip_grad_norm_`` before the update, inside the fused kernels (``DearEngine.norm_clip``; the norm
-    before clipping is ``engine.last_grad_norm``).
+    before clipping is ``engine.last_grad_norm``).  ``grad_comm_dtype=torch.bfloat16`` or ``torch.float16`` sends the
+    gradients of fp32 parameters to the reduce-scatter rounded to that dtype (``.to(dtype)`` on every rank, summed in
+    fp32): half the bytes over the link, like DDP's ``bf16_compress_hook`` / ``fp16_compress_hook``.  bf16 keeps fp32's
+    range; fp16 is meant to be paired with loss scaling (an overflow in the cast is an inf that ``GradScaler`` skips).
+    16-bit parameters and a single rank are unaffected.  ``compression=`` and ``fp16=`` are still ignored.
     """
     if threshold in (None, 0) and num_nearby_layers is None:
         threshold = float(os.environ.get("DEAR_THRESHOLD_MB", THRESHOLD))
@@ -848,7 +872,7 @@ def DistributedOptimizer(optimizer, model, compression=None, is_sparse=False, de
     opt = cls(optimizer.param_groups, model, threshold=threshold,
               num_nearby_layers=num_nearby_layers if num_nearby_layers is not None else NUM_NEARBY_LAYERS,
               exclude_parts=exclude_parts, policy=policy, verbose=verbose,
-              backward_passes_per_step=backward_passes_per_step)
+              backward_passes_per_step=backward_passes_per_step, grad_comm_dtype=grad_comm_dtype)
     if norm_clip is not None:
         opt._dear.norm_clip = norm_clip             # global-norm clipping of the averaged gradients
     if loss_scale is not None:

@@ -81,22 +81,26 @@ def measured_peaks(path: str = None) -> dict:
     return peaks
 
 
-def rs_roofline_us(bucket_bytes: int, world: int, elem_bytes: int = 4, peaks: dict = None) -> dict:
+def rs_roofline_us(bucket_bytes: int, world: int, elem_bytes: int = 4, peaks: dict = None,
+                   src_elem_bytes: int = None) -> dict:
     """Kernel A lower bound for one bucket on one GPU.
 
-    HBM: pack reads+writes the local bucket, the local shard is read, the fp32 shard is written;
-    NVLink: (P-1)/P of the bucket is pulled from peers (per direction).
+    HBM: pack reads the local gradients and writes the local bucket, the local shard is read, the fp32 shard is written;
+    NVLink: (P-1)/P of the bucket is pulled from peers (per direction).  ``bucket_bytes`` / ``elem_bytes`` describe the
+    bucket as it travels; ``src_elem_bytes`` (default ``elem_bytes``) is the gradient element the pack reads — 4 for
+    fp32 gradients sent at 16 bits (grad_comm_dtype).
     """
     pk = peaks or measured_peaks()
     shard = bucket_bytes / world
+    src_bytes = bucket_bytes / elem_bytes * (src_elem_bytes or elem_bytes)
     if world == 1 and elem_bytes == 4:
         hbm = 2 * bucket_bytes          # single GPU: the pack writes the fp32 shard directly
     else:
-        hbm = 2 * bucket_bytes + shard + (shard / elem_bytes) * 4
+        hbm = src_bytes + bucket_bytes + shard + (shard / elem_bytes) * 4
     link = bucket_bytes * (world - 1) / world
     t_hbm = hbm / (pk["hbm_gbs"] * 1e3)
     t_link = link / (pk["nvlink_gbs_per_dir"] * 1e3)
-    return {"hbm_us": t_hbm, "nvlink_us": t_link, "bound_us": max(t_hbm, t_link)}
+    return {"hbm_us": t_hbm, "nvlink_us": t_link, "bound_us": max(t_hbm, t_link), "hbm_bytes": hbm, "link_bytes": link}
 
 
 def ag_roofline_us(bucket_bytes: int, world: int, elem_bytes: int = 4, momentum: bool = True, peaks: dict = None) -> dict:

@@ -2,6 +2,7 @@
 """Micro-benchmark of the two fused kernels against their roofline and against NCCL.
 
     torchrun --nproc-per-node N tools/kernel_bench.py [--sizes-mb 1,4,16,24,64,392] [--dtype fp32]
+                                                      [--grad-comm-dtype fp32|bf16|fp16]
 
 For every bucket size it times (CUDA events, after warm-up, max over ranks)
   Kernel A  rs_kernel : pack + reduce-scatter + fp32 accumulate + 1/P scale
@@ -9,7 +10,10 @@ For every bucket size it times (CUDA events, after warm-up, max over ranks)
 and the NCCL collectives the reference issues for the same bucket
 (reduce_scatter_tensor / all_gather_into_tensor, without the reference's extra elementwise kernels).
 Bus bandwidth = bytes * (P-1)/P / time, reported against the H100 SXM data sheet's 450 GB/s per direction
-(utils/perf_model.py); at P = 1 the HBM roofline applies instead.
+(utils/perf_model.py); at P = 1 the HBM roofline applies instead.  ``--grad-comm-dtype bf16|fp16`` (fp32 buckets, P > 1)
+sends the gradients at 16 bits: the pack reads fp32 and writes 16-bit wire elements, the pull reads wire bytes.
+``rs_link_bytes`` / ``rs_hbm_bytes`` are the byte model of Kernel A per rank.  With ranks sharing one GPU, "peer" loads
+read local HBM, so those times say nothing about the link.
 """
 import argparse
 import json
@@ -31,6 +35,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sizes-mb", default="1,4,16,24,64,392")
     ap.add_argument("--dtype", default="fp32", choices=["fp32", "bf16"])
+    ap.add_argument("--grad-comm-dtype", default="fp32", choices=["fp32", "bf16", "fp16"],
+                    help="--dtype fp32 only: dtype of the gradient buckets (the pack rounds the fp32 gradients)")
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--nccl", type=int, default=1)
     ap.add_argument("--out", default=None)
@@ -45,7 +51,10 @@ def main():
     sizes_mb = [float(s) for s in args.sizes_mb.split(",")]
     quantum = world * 128 // es
     numels = [max(quantum, int(mb * 2 ** 20 / es) // quantum * quantum) for mb in sizes_mb]
-    bs = C.BucketSet(comm, numels, C.DT_F32 if args.dtype == "fp32" else C.DT_BF16, True)
+    wire = args.grad_comm_dtype if args.dtype == "fp32" and world > 1 and args.grad_comm_dtype != "fp32" else None
+    wes = 2 if wire else es                      # bytes per gradient element in the bucket (on the wire)
+    bs = C.BucketSet(comm, numels, C.DT_F32 if args.dtype == "fp32" else C.DT_BF16, True,
+                     {"bf16": C.DT_BF16, "fp16": C.DT_F16}.get(wire))
     results = []
     peaks = perf_model.measured_peaks()
 
@@ -73,22 +82,26 @@ def main():
 
     for g, n in enumerate(numels):
         nbytes = n * es
+        wbytes = n * wes
         shard = n // world
         grad_src = torch.randn(n, device=dev).to(tdt)                   # "autograd output" to be packed
         gs = torch.zeros(shard, device=dev)
         mom = torch.zeros(shard, device=dev)
         master = torch.zeros(shard, device=dev) if args.dtype != "fp32" else None
         bs.set_shards(g, gs, mom, master)
-        bs.set_pack(g, [grad_src.data_ptr()], [0], [nbytes], [0])
+        bs.set_pack(g, [grad_src.data_ptr()], [0], [wbytes], [0])
         bs.set_hyper(g, [n], [0.01], [1e-4], [0.9], [0.0], [0])
         bs.param_buffer(g).normal_()
         torch.cuda.synchronize()
         t_rs = timed(lambda: bs.reduce_scatter(g, True), args.iters)
         t_rs_nopack = timed(lambda: bs.reduce_scatter(g, False), args.iters)
         t_ag = timed(lambda: bs.allgather_update(g, True, False, True, False), args.iters)
-        row = {"bucket_mb": round(nbytes / 2 ** 20, 2), "dtype": args.dtype, "world": world, "rs_plan": bs.rs_plan(g),
+        row = {"bucket_mb": round(nbytes / 2 ** 20, 2), "dtype": args.dtype, "grad_comm_dtype": wire or args.dtype,
+               "world": world, "rs_plan": bs.rs_plan(g),
                "rs_us": round(t_rs, 2), "rs_nopack_us": round(t_rs_nopack, 2), "ag_sgd_us": round(t_ag, 2)}
-        rr = perf_model.rs_roofline_us(nbytes, world, es, peaks)
+        rr = perf_model.rs_roofline_us(wbytes, world, wes, peaks, src_elem_bytes=es)
+        row["rs_link_bytes"] = int(rr["link_bytes"])
+        row["rs_hbm_bytes"] = int(rr["hbm_bytes"])
         ar = perf_model.ag_roofline_us(nbytes, world, es, True, peaks)
         row["rs_roofline_us"] = round(rr["bound_us"], 2)
         row["ag_roofline_us"] = round(ar["bound_us"], 2)
@@ -96,7 +109,7 @@ def main():
         row["ag_frac_of_roofline"] = round(ar["bound_us"] / t_ag, 3)
         if world > 1:
             link = nbytes * (world - 1) / world
-            row["rs_busbw_gbs"] = round(link / t_rs / 1e3, 1)
+            row["rs_busbw_gbs"] = round(wbytes * (world - 1) / world / t_rs / 1e3, 1)
             row["ag_busbw_gbs"] = round(link / t_ag / 1e3, 1)
         if args.nccl and world > 1:
             full = torch.randn(n, device=dev).to(tdt)
