@@ -97,8 +97,9 @@ void rs_impl(const RSParams& p) {
       const uint64_t lo = uint64_t(k) * stripe_elems;
       const uint64_t hi = std::min<uint64_t>(p.shard_elems, lo + stripe_elems);
       for (uint64_t i = lo; i < hi; ++i) {
+        // the kernel's order: peers rank+1, ..., P-1, 0, ..., rank-1 first, my own bucket last (rs_pipe.cu producer)
         float acc = 0.f;
-        for (int q = 0; q < p.world; ++q) acc += ld<T>(p.grad.ptr[q], off + i);   // fixed order
+        for (int j = 0; j < p.world; ++j) acc += ld<T>(p.grad.ptr[(p.rank + 1 + j) % p.world], off + i);
         put(i, acc * scale);
       }
     }
