@@ -13,7 +13,7 @@ namespace py = pybind11;
 using namespace dear;
 
 namespace dear { namespace bn {
-bool bn_act_supported(const torch::Tensor& x);
+bool bn_act_supported(const torch::Tensor& x, const c10::optional<torch::Tensor>& residual);
 int64_t bn_act_launches();
 std::vector<torch::Tensor> bn_act_forward(const torch::Tensor& x, const c10::optional<torch::Tensor>& z,
                                           const c10::optional<torch::Tensor>& gamma, const c10::optional<torch::Tensor>& beta,
@@ -25,7 +25,9 @@ std::vector<torch::Tensor> bn_act_backward(const torch::Tensor& dy, const torch:
 } }
 
 namespace dear { namespace ln {
-bool ln_supported(const torch::Tensor& x);
+bool ln_supported(const torch::Tensor& x, const c10::optional<torch::Tensor>& residual,
+                  const c10::optional<torch::Tensor>& gamma, const c10::optional<torch::Tensor>& beta,
+                  const c10::optional<torch::Tensor>& a_bias);
 int64_t ln_launches();
 std::vector<torch::Tensor> ln_forward(const torch::Tensor& a, const torch::Tensor& residual, const torch::Tensor& gamma,
                                       const torch::Tensor& beta, double p, bool training, double eps,
@@ -33,7 +35,7 @@ std::vector<torch::Tensor> ln_forward(const torch::Tensor& a, const torch::Tenso
 std::vector<torch::Tensor> ln_backward(const torch::Tensor& dy, const torch::Tensor& s, const torch::Tensor& mean,
                                        const torch::Tensor& rstd, const torch::Tensor& gamma, const torch::Tensor& mask, double p,
                                        bool want_dbias);
-bool bias_gelu_supported(const torch::Tensor& z);
+bool bias_gelu_supported(const torch::Tensor& z, const c10::optional<torch::Tensor>& bias);
 torch::Tensor bias_gelu_forward(const torch::Tensor& z, const torch::Tensor& bias);
 std::vector<torch::Tensor> bias_gelu_backward(const torch::Tensor& dh, const torch::Tensor& z, const torch::Tensor& bias);
 } }
@@ -133,7 +135,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("comm_stream_handle", &BucketSet::comm_stream_handle);
 
   // fused channels-last BatchNorm (+ residual) (+ ReLU)
-  m.def("bn_act_supported", &dear::bn::bn_act_supported);
+  m.def("bn_act_supported", &dear::bn::bn_act_supported, py::arg("x"), py::arg("residual") = py::none());
   m.def("bn_act_launches", &dear::bn::bn_act_launches);
   m.def("bn_act_forward", &dear::bn::bn_act_forward, py::arg("x"), py::arg("residual"), py::arg("weight"), py::arg("bias"),
         py::arg("running_mean"), py::arg("running_var"), py::arg("training"), py::arg("momentum"), py::arg("eps"),
@@ -141,14 +143,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("bn_act_backward", &dear::bn::bn_act_backward);
 
   // fused dropout + residual add + LayerNorm
-  m.def("ln_supported", &dear::ln::ln_supported);
+  m.def("ln_supported", &dear::ln::ln_supported, py::arg("x"), py::arg("residual") = py::none(), py::arg("weight") = py::none(),
+        py::arg("bias") = py::none(), py::arg("a_bias") = py::none());
   m.def("ln_launches", &dear::ln::ln_launches);
   m.def("ln_forward", &dear::ln::ln_forward, py::arg("a"), py::arg("residual"), py::arg("weight"), py::arg("bias"),
         py::arg("p"), py::arg("training"), py::arg("eps"), py::arg("a_bias") = py::none());
   m.def("ln_backward", &dear::ln::ln_backward, py::arg("dy"), py::arg("s"), py::arg("mean"), py::arg("rstd"), py::arg("weight"),
         py::arg("mask"), py::arg("p"), py::arg("want_dbias") = false);
   // fused bias + GELU (forward) and GELU backward + bias gradient (backward)
-  m.def("bias_gelu_supported", &dear::ln::bias_gelu_supported);
+  m.def("bias_gelu_supported", &dear::ln::bias_gelu_supported, py::arg("z"), py::arg("bias") = py::none());
   m.def("bias_gelu_forward", &dear::ln::bias_gelu_forward);
   m.def("bias_gelu_backward", &dear::ln::bias_gelu_backward);
 

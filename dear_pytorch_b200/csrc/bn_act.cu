@@ -415,15 +415,20 @@ static bool make_geo(int64_t M, int64_t C, int vec, Geo* g) {
   return true;
 }
 
+// Every activation-sized operand moves as 128-bit vectors: a contiguous view at an odd storage offset is not one.
+static bool aligned16(const torch::Tensor& t) { return reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0; }
+
 static bool supported(const torch::Tensor& x) {
   if (!x.is_cuda() || x.dim() != 4) return false;
   if (x.scalar_type() != torch::kFloat && x.scalar_type() != torch::kBFloat16) return false;
-  if (!x.is_contiguous(at::MemoryFormat::ChannelsLast)) return false;
+  if (!x.is_contiguous(at::MemoryFormat::ChannelsLast) || !aligned16(x)) return false;
   Geo g;
   return make_geo(x.size(0) * x.size(2) * x.size(3), x.size(1), x.scalar_type() == torch::kFloat ? 4 : 8, &g);
 }
 
-bool bn_act_supported(const torch::Tensor& x) { return supported(x); }
+bool bn_act_supported(const torch::Tensor& x, const c10::optional<torch::Tensor>& residual) {
+  return supported(x) && (!residual.has_value() || aligned16(*residual));
+}
 
 template <typename T>
 static void fwd_impl(const torch::Tensor& x, const c10::optional<torch::Tensor>& z, const float* scale, const float* shift,
@@ -448,12 +453,17 @@ std::vector<torch::Tensor> bn_act_forward(const torch::Tensor& x, const c10::opt
                                           bool training, double momentum, double eps, bool relu) {
   TORCH_CHECK(supported(x), "bn_act_forward: unsupported input (need CUDA, 4-D channels_last, fp32/bf16, power-of-two width)");
   if (z.has_value()) TORCH_CHECK(z->sizes() == x.sizes() && z->scalar_type() == x.scalar_type() &&
-                                 z->is_contiguous(at::MemoryFormat::ChannelsLast), "residual must match x");
+                                 z->is_contiguous(at::MemoryFormat::ChannelsLast) && aligned16(*z),
+                                 "residual must match x (and be 16-byte aligned)");
+  const int64_t M = x.size(0) * x.size(2) * x.size(3);
+  // the variance of one value is undefined (and its unbiased form divides by zero); ops/fused_bn.py raises F.batch_norm's
+  // ValueError before it gets here
+  TORCH_CHECK(!training || M > 1, "bn_act_forward: Expected more than 1 value per channel when training");
   c10::cuda::CUDAGuard guard(x.device());
   cudaStream_t s = c10::cuda::getCurrentCUDAStream().stream();
   const bool f32 = x.scalar_type() == torch::kFloat;
   Geo g;
-  make_geo(x.size(0) * x.size(2) * x.size(3), x.size(1), f32 ? 4 : 8, &g);
+  make_geo(M, x.size(1), f32 ? 4 : 8, &g);
   const int C = g.C;
   auto fopt = x.options().dtype(torch::kFloat).memory_format(at::MemoryFormat::Contiguous);
   auto y = torch::empty_like(x);
@@ -519,9 +529,14 @@ std::vector<torch::Tensor> bn_act_backward(const torch::Tensor& dy_in, const tor
                                            const torch::Tensor& save_mean, const torch::Tensor& save_invstd,
                                            const torch::Tensor& scale, const torch::Tensor& shift, bool relu, bool has_residual) {
   TORCH_CHECK(supported(x), "bn_act_backward: unsupported input");
-  auto dy = dy_in.is_contiguous(at::MemoryFormat::ChannelsLast) ? dy_in : dy_in.contiguous(at::MemoryFormat::ChannelsLast);
-  TORCH_CHECK(dy.scalar_type() == x.scalar_type(), "grad dtype must match the input");
-  if (has_residual && relu) TORCH_CHECK(y.has_value(), "residual + ReLU backward needs the forward output");
+  auto dy = dy_in.is_contiguous(at::MemoryFormat::ChannelsLast) && aligned16(dy_in)
+                ? dy_in : dy_in.clone(at::MemoryFormat::ChannelsLast);
+  TORCH_CHECK(dy.scalar_type() == x.scalar_type() && dy.sizes() == x.sizes() && aligned16(dy),
+              "grad dtype and shape must match the input");
+  if (has_residual && relu)
+    TORCH_CHECK(y.has_value() && y->sizes() == x.sizes() && y->scalar_type() == x.scalar_type() &&
+                    y->is_contiguous(at::MemoryFormat::ChannelsLast) && aligned16(*y),
+                "residual + ReLU backward needs the forward output");
   c10::cuda::CUDAGuard guard(x.device());
   cudaStream_t s = c10::cuda::getCurrentCUDAStream().stream();
   const bool f32 = x.scalar_type() == torch::kFloat;

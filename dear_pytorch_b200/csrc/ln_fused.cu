@@ -380,12 +380,21 @@ bias_gelu_bwd_kernel(const T* __restrict__ dh, const T* __restrict__ z, const T*
 }
 
 // ------------------------------------------------------------------------------------------- host
-bool ln_supported(const torch::Tensor& x) {
-  if (!x.is_cuda() || x.dim() < 2) return false;
+// Every operand the kernels read or write moves as 128-bit vectors: a contiguous view at an odd storage offset is not one.
+static bool aligned16(const torch::Tensor& t) { return reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0; }
+static bool aligned16(const c10::optional<torch::Tensor>& t) { return !t.has_value() || aligned16(*t); }
+
+static bool ln_shape_ok(const torch::Tensor& x) {
+  if (!x.is_cuda() || x.dim() < 2 || !aligned16(x)) return false;
   const int64_t H = x.size(-1);
   if (x.scalar_type() == at::kBFloat16) return H % 8 == 0 && H <= kMaxCols;
   if (x.scalar_type() == at::kFloat) return H % 4 == 0 && H <= kMaxCols;
   return false;
+}
+
+bool ln_supported(const torch::Tensor& x, const c10::optional<torch::Tensor>& residual, const c10::optional<torch::Tensor>& gamma,
+                  const c10::optional<torch::Tensor>& beta, const c10::optional<torch::Tensor>& a_bias) {
+  return ln_shape_ok(x) && aligned16(residual) && aligned16(gamma) && aligned16(beta) && aligned16(a_bias);
 }
 
 static int grid_for(int rows, int ctas_per_sm) {
@@ -428,7 +437,8 @@ static void fwd_launch(const torch::Tensor& a, const c10::optional<torch::Tensor
 std::vector<torch::Tensor> ln_forward(const torch::Tensor& a, const torch::Tensor& residual, const torch::Tensor& gamma,
                                       const torch::Tensor& beta, double p, bool training, double eps,
                                       const c10::optional<torch::Tensor>& a_bias) {
-  TORCH_CHECK(ln_supported(a), "dropout_add_layer_norm: unsupported tensor (CUDA bf16 with H % 8 == 0 or fp32 with H % 4 == 0, H <= 1024)");
+  TORCH_CHECK(ln_supported(a, residual, gamma, beta, a_bias),
+              "dropout_add_layer_norm: unsupported tensor (16-byte aligned CUDA bf16 with H % 8 == 0 or fp32 with H % 4 == 0, H <= 1024)");
   TORCH_CHECK(a.is_contiguous() && residual.is_contiguous() && gamma.is_contiguous() && beta.is_contiguous(),
               "dropout_add_layer_norm: contiguous tensors expected");
   TORCH_CHECK(a.sizes() == residual.sizes() && a.scalar_type() == residual.scalar_type() &&
@@ -493,7 +503,9 @@ static void bwd_launch(const torch::Tensor& dy, const torch::Tensor& s, const to
 std::vector<torch::Tensor> ln_backward(const torch::Tensor& dy, const torch::Tensor& s, const torch::Tensor& mean,
                                        const torch::Tensor& rstd, const torch::Tensor& gamma, const torch::Tensor& mask, double p,
                                        bool want_dbias) {
-  TORCH_CHECK(ln_supported(dy) && dy.is_contiguous() && s.is_contiguous(), "dropout_add_layer_norm backward: unsupported tensor");
+  TORCH_CHECK(ln_supported(dy, s, gamma, c10::nullopt, c10::nullopt) && dy.is_contiguous() && s.is_contiguous() &&
+                  s.sizes() == dy.sizes() && s.scalar_type() == dy.scalar_type(),
+              "dropout_add_layer_norm backward: unsupported tensor");
   c10::cuda::CUDAGuard guard(dy.device());
   const int H = dy.size(-1);
   const int rows = dy.numel() / H;
@@ -517,11 +529,13 @@ std::vector<torch::Tensor> ln_backward(const torch::Tensor& dy, const torch::Ten
 
 // ---- bias + GELU ------------------------------------------------------------------------------------
 static bool bg_supported(const torch::Tensor& z) {
-  if (!z.is_cuda() || z.dim() < 2 || !z.is_contiguous()) return false;
+  if (!z.is_cuda() || z.dim() < 2 || !z.is_contiguous() || !aligned16(z)) return false;
   const int64_t N = z.size(-1);
   return (z.scalar_type() == at::kBFloat16 && N % 8 == 0) || (z.scalar_type() == at::kFloat && N % 4 == 0);
 }
-bool bias_gelu_supported(const torch::Tensor& z) { return bg_supported(z); }
+bool bias_gelu_supported(const torch::Tensor& z, const c10::optional<torch::Tensor>& bias) {
+  return bg_supported(z) && aligned16(bias);
+}
 
 static dim3 bg_grid(int rows, int N, int vec) {
   const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
@@ -532,7 +546,8 @@ static dim3 bg_grid(int rows, int N, int vec) {
 
 torch::Tensor bias_gelu_forward(const torch::Tensor& z, const torch::Tensor& bias) {
   TORCH_CHECK(bg_supported(z), "bias_gelu: unsupported tensor (contiguous CUDA bf16 / fp32, last dim a multiple of one 128-bit vector)");
-  TORCH_CHECK(bias.is_contiguous() && bias.numel() == z.size(-1) && bias.scalar_type() == z.scalar_type(), "bias_gelu: bias");
+  TORCH_CHECK(bias.is_contiguous() && aligned16(bias) && bias.numel() == z.size(-1) && bias.scalar_type() == z.scalar_type(),
+              "bias_gelu: bias");
   c10::cuda::CUDAGuard guard(z.device());
   const int N = z.size(-1);
   const int rows = z.numel() / N;
@@ -554,8 +569,10 @@ torch::Tensor bias_gelu_forward(const torch::Tensor& z, const torch::Tensor& bia
 
 // returns {dz, dbias}
 std::vector<torch::Tensor> bias_gelu_backward(const torch::Tensor& dh, const torch::Tensor& z, const torch::Tensor& bias) {
-  TORCH_CHECK(bg_supported(z) && dh.is_contiguous() && dh.sizes() == z.sizes() && dh.scalar_type() == z.scalar_type(),
+  TORCH_CHECK(bg_supported(z) && dh.is_contiguous() && aligned16(dh) && dh.sizes() == z.sizes() && dh.scalar_type() == z.scalar_type(),
               "bias_gelu backward: unsupported tensors");
+  TORCH_CHECK(bias.is_contiguous() && aligned16(bias) && bias.numel() == z.size(-1) && bias.scalar_type() == z.scalar_type(),
+              "bias_gelu backward: bias");
   c10::cuda::CUDAGuard guard(z.device());
   const int N = z.size(-1);
   const int rows = z.numel() / N;

@@ -23,8 +23,8 @@ class _BiasGelu(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dh):
         z, bias = ctx.saved_tensors
-        if not dh.is_contiguous():
-            dh = dh.contiguous()
+        if not dh.is_contiguous() or dh.data_ptr() % 16:
+            dh = dh.clone(memory_format=torch.contiguous_format)
         dz, dbias = native().bias_gelu_backward(dh, z, bias)
         return dz, (dbias if ctx.needs_input_grad[1] else None)
 
@@ -32,7 +32,7 @@ class _BiasGelu(torch.autograd.Function):
 def bias_gelu(z: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
     """``gelu(z + bias)`` (erf form) with the bias gradient fused into the backward."""
     C = native()
-    if (C is not None and z.is_cuda and hasattr(C, "bias_gelu_supported") and C.bias_gelu_supported(z)
+    if (C is not None and z.is_cuda and hasattr(C, "bias_gelu_supported") and C.bias_gelu_supported(z, bias)
             and bias.dtype == z.dtype and bias.is_contiguous()):
         return _BiasGelu.apply(z, bias)
     return F.gelu(z + bias)

@@ -4,8 +4,8 @@
 keys) whose forward is ``act(bn(x) [+ residual])`` in ONE pass over the activations
 (csrc/bn_act.cu): 8 tensor passes per layer and iteration instead of ~13 for
 ``BatchNorm2d -> (+) -> ReLU`` as separate cuDNN / ATen kernels.  On inputs the kernels do not
-cover (CPU, NCHW, widths that are not a power-of-two number of 128-bit vectors, bf16 affine
-parameters, eval-mode backward) it falls back to the equivalent PyTorch composite, so a model
+cover (CPU, NCHW, widths that are not a power-of-two number of 128-bit vectors, views that are not
+16-byte aligned, bf16 affine parameters, eval-mode backward) it falls back to the equivalent PyTorch composite, so a model
 using it runs everywhere.
 """
 from __future__ import annotations
@@ -50,15 +50,19 @@ def bn_act(x: torch.Tensor, weight, bias, running_mean, running_var, training: b
            relu: bool = True, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Functional form.  Uses the fused kernels when they apply, else the PyTorch composite."""
     C = native()
-    ok = (C is not None and x.is_cuda and momentum is not None and C.bn_act_supported(x)
+    ok = (C is not None and x.is_cuda and momentum is not None and C.bn_act_supported(x, residual)
           and (weight is None or weight.dtype == torch.float32) and (bias is None or bias.dtype == torch.float32)
           and (residual is None or (residual.dtype == x.dtype and residual.shape == x.shape
                                     and residual.is_contiguous(memory_format=torch.channels_last))))
     if ok and training:
+        if x.numel() == x.size(1):                    # what F.batch_norm raises: one value per channel has no variance
+            raise ValueError("Expected more than 1 value per channel when training, got input size {}".format(x.size()))
         return _BNActFunction.apply(x, residual, weight, bias, running_mean, running_var, float(momentum), float(eps), relu)
     if ok and not torch.is_grad_enabled() and running_mean is not None:
         return C.bn_act_forward(x, residual, weight, bias, running_mean, running_var, False, float(momentum), float(eps),
                                 relu)[0]
+    if x.is_cuda and x.data_ptr() % 16:
+        x = x.clone()                                  # cuDNN's batch norm loads 16-byte vectors too
     return _composite(x, residual, weight, bias, running_mean, running_var, training, momentum, eps, relu)
 
 

@@ -7,8 +7,8 @@ in one kernel forward and one (+ a tiny column reduction) backward instead of th
 ATen kernels.  ``FusedDropoutAddLayerNorm`` is a drop-in ``nn.LayerNorm`` (same parameters and
 state-dict keys) with a ``forward(a, residual)``.
 
-The kernels cover CUDA tensors in fp32 / bf16 with a hidden size up to 1024 that is a multiple of
-one 128-bit vector; anything else takes the PyTorch composite, which is also the numerics reference.
+The kernels cover 16-byte aligned CUDA tensors in fp32 / bf16 with a hidden size up to 1024 that is a
+multiple of one 128-bit vector; anything else takes the PyTorch composite, which is also the numerics reference.
 """
 from __future__ import annotations
 
@@ -31,8 +31,8 @@ class _DropAddLN(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         s, mean, rstd, weight, mask = ctx.saved_tensors
-        if not dy.is_contiguous():
-            dy = dy.contiguous()
+        if not dy.is_contiguous() or dy.data_ptr() % 16:
+            dy = dy.clone(memory_format=torch.contiguous_format)
         want_dbias = ctx.has_branch_bias and ctx.needs_input_grad[7]
         d_res, d_a, dgamma, dbeta, dbias = native().ln_backward(dy, s, mean, rstd, weight, mask, ctx.p, want_dbias)
         return (d_a if ctx.needs_input_grad[0] else None, d_res if ctx.needs_input_grad[1] else None,
@@ -46,10 +46,10 @@ def _composite(a, residual, weight, bias, p, training, eps, branch_bias=None):
     return F.layer_norm(residual + F.dropout(a, p, training), (a.shape[-1],), weight, bias, eps)
 
 
-def fused_ln_applicable(a: torch.Tensor, residual: torch.Tensor, weight, bias) -> bool:
+def fused_ln_applicable(a: torch.Tensor, residual: torch.Tensor, weight, bias, branch_bias=None) -> bool:
     C = native()
     return (C is not None and a.is_cuda and weight is not None and bias is not None and hasattr(C, "ln_supported")
-            and C.ln_supported(a) and a.shape == residual.shape and a.dtype == residual.dtype == weight.dtype == bias.dtype
+            and C.ln_supported(a, residual, weight, bias, branch_bias) and a.shape == residual.shape and a.dtype == residual.dtype == weight.dtype == bias.dtype
             and a.is_contiguous() and residual.is_contiguous())
 
 
@@ -65,7 +65,7 @@ def dropout_add_layer_norm(a, residual, weight, bias, p: float = 0.0, training: 
         a = a.contiguous()
     if residual.is_cuda and not residual.is_contiguous():
         residual = residual.contiguous()
-    if fused_ln_applicable(a, residual, weight, bias) and (
+    if fused_ln_applicable(a, residual, weight, bias, branch_bias) and (
             branch_bias is None or (branch_bias.dtype == a.dtype and branch_bias.is_contiguous())):
         return _DropAddLN.apply(a, residual, weight, bias, float(p), bool(training), float(eps), branch_bias)
     return _composite(a, residual, weight, bias, p, training, eps, branch_bias)
