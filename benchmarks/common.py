@@ -46,8 +46,12 @@ def add_common_args(ap):
                     help="sparse WFBP: accumulate the velocity before sparsification (wfbp/dopt.py:906-953)")
     ap.add_argument("--exclude-parts", type=str, default="", help="reducescatter, allgather (time breakdown)")
     ap.add_argument("--momentum", type=float, default=0.0)
-    ap.add_argument("--optimizer", choices=["sgd", "adam", "adamw"], default="sgd",
-                    help="adam/adamw: sharded Adam fused into the all-gather kernel (dear methods only)")
+    ap.add_argument("--optimizer", choices=["sgd", "adam", "adamw", "rmsprop"], default="sgd",
+                    help="adam/adamw/rmsprop: sharded Adam / RMSprop fused into the all-gather kernel (dear methods only); "
+                         "RMSprop takes its momentum from --momentum")
+    ap.add_argument("--rmsprop-alpha", type=float, default=0.99, help="--optimizer rmsprop: smoothing constant alpha")
+    ap.add_argument("--rmsprop-eps", type=float, default=1e-8, help="--optimizer rmsprop: eps")
+    ap.add_argument("--rmsprop-centered", action="store_true", default=False, help="--optimizer rmsprop: centered")
     ap.add_argument("--graph", type=int, default=0, help="capture the whole iteration in a CUDA graph")
     ap.add_argument("--norm-clip", type=float, default=None,
                     help="dear, dear-bo, dear-notf: clip the global gradient norm to this value (clip_grad_norm_ semantics, "
@@ -206,4 +210,7 @@ def make_base_optimizer(args, params, lr):
         return torch.optim.AdamW(params, lr=lr)
     if getattr(args, "optimizer", "sgd") == "adam":
         return torch.optim.Adam(params, lr=lr)
+    if getattr(args, "optimizer", "sgd") == "rmsprop":
+        return torch.optim.RMSprop(params, lr=lr, alpha=args.rmsprop_alpha, eps=args.rmsprop_eps, momentum=args.momentum,
+                                   centered=args.rmsprop_centered)
     return torch.optim.SGD(params, lr=lr, momentum=args.momentum)

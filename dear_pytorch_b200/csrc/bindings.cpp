@@ -111,7 +111,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("param_buffer", &BucketSet::param_buffer)
       .def("grad_buffer", &BucketSet::grad_buffer)
       .def("set_shards", &BucketSet::set_shards, py::arg("bucket"), py::arg("grad_shard"),
-           py::arg("momentum") = py::none(), py::arg("master") = py::none(), py::arg("var") = py::none())
+           py::arg("momentum") = py::none(), py::arg("master") = py::none(), py::arg("var") = py::none(),
+           py::arg("grad_avg") = py::none())
       .def("set_step", &BucketSet::set_step)
       .def("set_pack", &BucketSet::set_pack)
       .def("set_hyper", &BucketSet::set_hyper, py::arg("bucket"), py::arg("ends"), py::arg("lr"), py::arg("weight_decay"),
@@ -160,6 +161,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("OPT_SGD") = static_cast<int>(OPT_SGD);
   m.attr("OPT_ADAM") = static_cast<int>(OPT_ADAM);
   m.attr("OPT_ADAMW") = static_cast<int>(OPT_ADAMW);
+  m.attr("OPT_RMSPROP") = static_cast<int>(OPT_RMSPROP);
+  m.attr("HYPER_NESTEROV") = static_cast<int>(HYPER_NESTEROV);
+  m.attr("HYPER_SKIP") = static_cast<int>(HYPER_SKIP);
+  m.attr("HYPER_CENTERED") = static_cast<int>(HYPER_CENTERED);
   m.attr("DT_F32") = static_cast<int>(DT_F32);
   m.attr("DT_BF16") = static_cast<int>(DT_BF16);
   m.attr("DT_F16") = static_cast<int>(DT_F16);

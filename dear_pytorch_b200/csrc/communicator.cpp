@@ -507,7 +507,8 @@ void BucketSet::set_step(int g, int64_t t) {
 }
 
 void BucketSet::set_shards(int g, torch::Tensor grad_shard, std::optional<torch::Tensor> mom,
-                           std::optional<torch::Tensor> master, std::optional<torch::Tensor> var) {
+                           std::optional<torch::Tensor> master, std::optional<torch::Tensor> var,
+                           std::optional<torch::Tensor> grad_avg) {
   auto& b = buckets_.at(g);
   auto chk = [&](const torch::Tensor& t, const char* what) {
     DEAR_CHECK(t.scalar_type() == torch::kFloat && t.is_contiguous() && t.numel() == b.shard,
@@ -522,6 +523,8 @@ void BucketSet::set_shards(int g, torch::Tensor grad_shard, std::optional<torch:
   if (master.has_value() && master->defined()) { chk(*master, "master shard"); b.master = *master; }
   b.var = torch::Tensor();
   if (var.has_value() && var->defined()) { chk(*var, "second-moment shard"); b.var = *var; }
+  b.gavg = torch::Tensor();
+  if (grad_avg.has_value() && grad_avg->defined()) { chk(*grad_avg, "grad_avg shard"); b.gavg = *grad_avg; }
   // (low-precision buckets must have a master shard by the time allgather_update() runs)
 }
 
@@ -690,7 +693,7 @@ bool BucketSet::set_hyper(int g, const std::vector<int64_t>& ends, const std::ve
     segs[i].weight_decay = static_cast<float>(wd[i]);
     segs[i].momentum = static_cast<float>(mom[i]);
     segs[i].dampening = static_cast<float>(damp[i]);
-    segs[i].nesterov = static_cast<uint32_t>(nesterov[i]) & (HYPER_NESTEROV | HYPER_SKIP);
+    segs[i].nesterov = static_cast<uint32_t>(nesterov[i]) & (HYPER_NESTEROV | HYPER_SKIP | HYPER_CENTERED);
     segs[i].opt = i < opt.size() ? static_cast<uint32_t>(opt[i]) : OPT_SGD;
     segs[i].beta2 = i < beta2.size() ? static_cast<float>(beta2[i]) : 0.f;
     segs[i].eps = i < eps.size() ? static_cast<float>(eps[i]) : 0.f;
@@ -699,10 +702,21 @@ bool BucketSet::set_hyper(int g, const std::vector<int64_t>& ends, const std::ve
   DEAR_CHECK(segs.back().end >= static_cast<uint64_t>(b.padded), "set_hyper: segments must cover the bucket");
   const bool same = segs.size() == b.hyper_host.size() &&
                     std::memcmp(segs.data(), b.hyper_host.data(), segs.size() * sizeof(HyperSeg)) == 0;
-  bool any_adam = false, all_adam = true;
-  for (const auto& sg : segs) { any_adam |= sg.opt != OPT_SGD; all_adam &= sg.opt != OPT_SGD; }
+  bool any_adam = false, all_adam = true, any_rms = false, all_rms = true, rms_mom = false, rms_centered = false;
+  for (const auto& sg : segs) {
+    const bool adam = sg.opt == OPT_ADAM || sg.opt == OPT_ADAMW, rms = sg.opt == OPT_RMSPROP;
+    DEAR_CHECK(sg.opt <= OPT_RMSPROP, "set_hyper: unknown optimizer kind " << sg.opt);
+    any_adam |= adam; all_adam &= adam;
+    any_rms |= rms; all_rms &= rms;
+    rms_mom |= rms && sg.momentum > 0.f;
+    rms_centered |= rms && (sg.nesterov & HYPER_CENTERED) != 0;
+  }
   DEAR_CHECK(!any_adam || all_adam, "a bucket cannot mix SGD and Adam parameter groups");
+  DEAR_CHECK(!any_rms || all_rms, "a bucket cannot mix RMSprop with other optimizers' parameter groups");
   b.adam = all_adam;
+  b.rmsprop = all_rms;
+  b.rms_momentum = rms_mom;
+  b.rms_centered = rms_centered;
   if (same) return false;
   b.hyper_host = std::move(segs);
   if (comm_->is_cuda())
@@ -857,6 +871,15 @@ void BucketSet::allgather_update(int g, bool do_update, bool first_step, bool en
     if (b.adam) {
       DEAR_CHECK(b.mom.defined() && b.var.defined(), "Adam needs exp_avg and exp_avg_sq shards (set_shards)");
       p.var_shard = b.var.data_ptr<float>();
+    }
+    p.rmsprop = b.rmsprop ? 1u : 0u;
+    if (b.rmsprop) {
+      DEAR_CHECK(b.var.defined(), "RMSprop needs a square_avg shard (set_shards var)");
+      DEAR_CHECK(!b.rms_momentum || b.mom.defined(), "RMSprop with momentum needs a momentum_buffer shard (set_shards)");
+      DEAR_CHECK(!b.rms_centered || b.gavg.defined(), "centered RMSprop needs a grad_avg shard (set_shards)");
+      p.var_shard = b.var.data_ptr<float>();
+      p.gavg_shard = b.rms_centered ? b.gavg.data_ptr<float>() : nullptr;
+      if (!b.rms_momentum) p.mom_shard = nullptr;
     }
     p.step_ctr = arena_->ctrl() + 2 * kNumChannels + g;
     p.hyper = cuda ? b.hyper_dev : b.hyper_host.data();

@@ -132,8 +132,11 @@ class BucketSet {
   bool has_multicast() const { return arena_->has_multicast(); }
   bool converting() const { return gdtype_ != dtype_; }
 
+  // optimizer state shards of bucket g: momentum (SGD / RMSprop buffer, Adam exp_avg), var (Adam exp_avg_sq, RMSprop
+  // square_avg), grad_avg (centered RMSprop); absent ones as None
   void set_shards(int g, torch::Tensor grad_shard, std::optional<torch::Tensor> mom,
-                  std::optional<torch::Tensor> master, std::optional<torch::Tensor> var);
+                  std::optional<torch::Tensor> master, std::optional<torch::Tensor> var,
+                  std::optional<torch::Tensor> grad_avg = std::nullopt);
   // number of updates already applied to bucket g (Adam bias correction); device-resident afterwards
   void set_step(int g, int64_t t);
   // Gradient sources for the fused pack.  Returns true if the device table was re-uploaded.
@@ -173,8 +176,11 @@ class BucketSet {
     int64_t padded = 0;
     int64_t shard = 0;
     size_t param_off = 0, grad_off = 0;
-    torch::Tensor grad_shard, mom, master, var;
+    torch::Tensor grad_shard, mom, master, var, gavg;
     bool adam = false;
+    bool rmsprop = false;
+    bool rms_momentum = false;            // some RMSprop segment has momentum > 0: needs the momentum shard
+    bool rms_centered = false;            // some RMSprop segment is centered: needs the grad_avg shard
     std::vector<PackSeg> pack_host;
     std::vector<HyperSeg> hyper_host;
     uint32_t ntiles = 0;

@@ -85,23 +85,30 @@ struct PackSeg {
 constexpr uint32_t SEG_ZERO_FILL = 1u;
 
 // Contiguous element range of a bucket sharing one set of optimizer hyper-parameters.
-enum OptKind : uint32_t { OPT_SGD = 0, OPT_ADAM = 1 /* L2 in the gradient */, OPT_ADAMW = 2 /* decoupled decay */ };
+enum OptKind : uint32_t {
+  OPT_SGD = 0,
+  OPT_ADAM = 1 /* L2 in the gradient */,
+  OPT_ADAMW = 2 /* decoupled decay */,
+  OPT_RMSPROP = 3 /* torch.optim.RMSprop, L2 in the gradient */
+};
 struct HyperSeg {
   uint64_t end;           // exclusive end (element offset within the bucket)
   float lr;
   float weight_decay;
-  float momentum;         // SGD momentum, or Adam beta1
-  float dampening;
+  float momentum;         // SGD / RMSprop momentum, or Adam beta1
+  float dampening;        // SGD dampening; RMSprop: 1 - alpha (rounded once from double, as torch passes it)
   uint32_t nesterov;      // bit0: Nesterov momentum; bit1 (HYPER_SKIP): this rank saw no gradient for the range in
                           // this step — where the REDUCED gradient is exactly zero too (absent on every rank), leave
-                          // parameter and state untouched, like torch.optim skips ``p.grad is None``
+                          // parameter and state untouched, like torch.optim skips ``p.grad is None``;
+                          // bit2 (HYPER_CENTERED): centered RMSprop
   uint32_t opt;           // OptKind
-  float beta2;            // Adam only
-  float eps;              // Adam only
+  float beta2;            // Adam beta2; RMSprop alpha
+  float eps;              // Adam / RMSprop
 };
 
 constexpr uint32_t HYPER_NESTEROV = 1u;
 constexpr uint32_t HYPER_SKIP = 2u;
+constexpr uint32_t HYPER_CENTERED = 4u;
 
 // ---- per-element math shared by the CUDA kernels and the host emulation ----
 
@@ -141,6 +148,33 @@ DEAR_HD float adam_update(float p, float g, float& m, float& v, const HyperSeg& 
 #endif
   if (h.opt == OPT_ADAMW) p = p * (1.f - h.lr * h.weight_decay);
   return p - (h.lr / bc1) * (m / denom);
+}
+
+// torch.optim.RMSprop semantics (torch/optim/rmsprop.py, _single_tensor_rmsprop): square_avg `sq`, grad_avg `ga`
+// (centered only), momentum_buffer `buf` (momentum > 0 only), all starting at zero — there is no first-step rule, and
+// the step count changes nothing.  `w` = h.dampening = 1 - alpha.  grad_avg.lerp_(g, w) is ATen's lerp (Lerp.h), both
+// branches.  The centered variance is not clamped: a negative difference gives NaN, as in torch.
+DEAR_HD float rmsprop_update(float p, float g, float& sq, float& ga, float& buf, const HyperSeg& h, float coef) {
+  if ((h.nesterov & HYPER_SKIP) && g == 0.f) return p;
+  g = g * coef;                                    // clipping coefficient, as in sgd_update
+  if (h.weight_decay != 0.f) g = g + h.weight_decay * p;
+  const float w = h.dampening;
+  sq = h.beta2 * sq + w * g * g;
+  float v = sq;
+  if (h.nesterov & HYPER_CENTERED) {
+    ga = (w < 0.5f && w > -0.5f) ? ga + w * (g - ga) : g - (g - ga) * (1.f - w);
+    v = sq - ga * ga;
+  }
+#if defined(__CUDA_ARCH__)
+  const float avg = sqrtf(v) + h.eps;
+#else
+  const float avg = std::sqrt(v) + h.eps;
+#endif
+  if (h.momentum > 0.f) {
+    buf = h.momentum * buf + g / avg;
+    return p - h.lr * buf;
+  }
+  return p - h.lr * (g / avg);
 }
 
 // Index of the hyper segment containing element `e` (segments sorted by end).
@@ -325,6 +359,10 @@ struct AGParams {
   // global-norm clipping (nullptr => none): the deciding kernel forms clip->total_norm and clip->coef from every rank's
   // partial sum of squares; every update kernel of the step multiplies clip->coef into the gradient
   ClipState* clip;
+  // RMSprop (every hyper segment is OPT_RMSPROP): var_shard is square_avg, mom_shard the momentum buffer (nullptr when
+  // no segment has momentum), gavg_shard grad_avg (nullptr when no segment is centered)
+  uint32_t rmsprop;
+  float* gavg_shard;
 };
 
 // AG_ARRIVE flag encoding: (epoch << 1) | overflow bit of the sender (0 unless it is the deciding kernel).

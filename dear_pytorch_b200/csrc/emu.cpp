@@ -209,6 +209,13 @@ void ag_impl(const AGParams& p) {
         const float bc1 = 1.f - std::pow(h.momentum, float(t_step));
         const float sqrt_bc2 = std::sqrt(1.f - std::pow(h.beta2, float(t_step)));
         pv = adam_update(pv, p.grad_shard[i], p.mom_shard[i], p.var_shard[i], h, bc1, sqrt_bc2, coef);
+      } else if (p.rmsprop) {
+        // absent shards are neither read nor written (no segment of the bucket uses them)
+        float mv = has_mom ? p.mom_shard[i] : 0.f;
+        float av = p.gavg_shard ? p.gavg_shard[i] : 0.f;
+        pv = rmsprop_update(pv, p.grad_shard[i], p.var_shard[i], av, mv, h, coef);
+        if (has_mom && h.momentum > 0.f) p.mom_shard[i] = mv;
+        if (p.gavg_shard && (h.nesterov & HYPER_CENTERED)) p.gavg_shard[i] = av;
       } else {
         float mv = (has_mom && !first_step) ? p.mom_shard[i] : 0.f;
         pv = sgd_update(pv, p.grad_shard[i], mv, h, first_step, has_mom, coef);

@@ -3,7 +3,7 @@
 // Kernel A (rs_kernel):   gradient pack + reduce-scatter + fp32 accumulate + 1/P scale
 //                         replaces: bucket copy_ (dear/dear_dopt.py:265), ncclReduceScatter
 //                         (common/comm_core/src/communicator.cpp:157-169) and div_ (:306).
-// Kernel B (ag_kernel):   sharded SGD/momentum update + all-gather (push) of the updated
+// Kernel B (ag_kernel):   sharded SGD/momentum, Adam/AdamW or RMSprop update + all-gather (push) of the updated
 //                         parameter shard, replaces ncclAllGather (communicator.cpp:171-183),
 //                         the copy-out / div_ / _sgd / fill_ per-parameter loop
 //                         (dear/dear_dopt.py:293-336).
@@ -354,14 +354,20 @@ __device__ __forceinline__ void st_f32x(float* base, uint64_t v, int ev, const f
   if (ev == 8) m[1] = make_float4(in[4], in[5], in[6], in[7]);
 }
 
+// OPT: the optimizer family of every hyper segment (AG_SGD also serves a pure all-gather).  Each is its own
+// instantiation, so adding one leaves the code of the others as it was.
+enum AgOpt : int { AG_SGD = 0, AG_ADAM = 1 /* Adam and AdamW */, AG_RMSPROP = 2 };
 // CLIP: global-norm clipping (p.clip != nullptr): multiply the step's coefficient into the gradient.  A separate
 // instantiation, so the path without clipping compiles as before.
-template <typename T, int W, bool MC, bool ADAM, bool CLIP>
+template <typename T, int W, bool MC, int OPT, bool CLIP>
 __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
   using Tr = ElemTraits<T>;
+  constexpr bool ADAM = OPT == AG_ADAM;
+  constexpr bool RMS = OPT == AG_RMSPROP;       // square_avg in vv, grad_avg in av, momentum buffer in mv
   constexpr int EV = Tr::kPerVec;
   constexpr int EVA = 8;                        // register array length (>= EV)
-  constexpr int U = ADAM ? ((EV == 4) ? 2 : 1) : ((EV == 4) ? 4 : 2);   // vectors in flight per thread
+  // vectors in flight per thread; centered RMSprop with momentum streams five fp32 arrays, like Adam's four plus one
+  constexpr int U = (ADAM || RMS) ? ((EV == 4) ? 2 : 1) : ((EV == 4) ? 4 : 2);
   __shared__ HyperSeg s_hyper[kMaxSmemHyper];
 
   const int tid = threadIdx.x;
@@ -457,12 +463,14 @@ __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
     const uint64_t gstride = uint64_t(gridDim.x) * kThreads;
     const char* local_param = reinterpret_cast<const char*>(p.param.ptr[p.rank]);
     const bool has_mom = p.mom_shard != nullptr;
-    const bool load_mom = has_mom && (ADAM || !first_step) && upd;
+    const bool load_mom = has_mom && (ADAM || RMS || !first_step) && upd;   // RMSprop's buffer starts at zero
+    const bool has_gavg = RMS && p.gavg_shard != nullptr;
     // Adam bias corrections come from a device-resident update counter (graph replay safe)
     const uint32_t t_step = (ADAM && p.step_ctr != nullptr) ? *reinterpret_cast<volatile uint32_t*>(p.step_ctr) + 1 : 1;
     for (uint64_t v0 = uint64_t(blockIdx.x) * kThreads + tid; v0 < nvec; v0 += gstride * U) {
       float pv[U][EVA], gv[U][EVA], mv[U][EVA];
-      float vv[ADAM ? U : 1][EVA];
+      float vv[(ADAM || RMS) ? U : 1][EVA];
+      float av[RMS ? U : 1][EVA];
       // ---- all loads first (memory-level parallelism) ----
 #pragma unroll
       for (int u = 0; u < U; ++u) {
@@ -481,6 +489,15 @@ __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
             for (int k = 0; k < EV; ++k) mv[u][k] = 0.f;
           }
           if (ADAM && upd) ld_f32x(p.var_shard, v, EV, vv[ADAM ? u : 0]);
+          if (RMS && upd) ld_f32x(p.var_shard, v, EV, vv[RMS ? u : 0]);
+          if (RMS) {
+            if (has_gavg && upd) {
+              ld_f32x(p.gavg_shard, v, EV, av[RMS ? u : 0]);
+            } else {
+#pragma unroll
+              for (int k = 0; k < EV; ++k) av[RMS ? u : 0][k] = 0.f;
+            }
+          }
         }
       }
       // ---- update + stores ----
@@ -500,6 +517,14 @@ __global__ void __launch_bounds__(kThreads, 1) ag_kernel(const AGParams p) {
                                        CLIP ? coef : 1.f);
               st_f32x(p.mom_shard, v, EV, mv[u]);
               st_f32x(p.var_shard, v, EV, vv[ADAM ? u : 0]);
+            } else if (RMS) {
+              const int r = RMS ? u : 0;
+#pragma unroll
+              for (int k = 0; k < EV; ++k)
+                pv[u][k] = rmsprop_update(pv[u][k], gv[u][k], vv[r][k], av[r][k], mv[u][k], h, CLIP ? coef : 1.f);
+              st_f32x(p.var_shard, v, EV, vv[r]);
+              if (has_mom && h.momentum > 0.f) st_f32x(p.mom_shard, v, EV, mv[u]);
+              if (has_gavg && (h.nesterov & HYPER_CENTERED)) st_f32x(p.gavg_shard, v, EV, av[r]);
             } else {
 #pragma unroll
               for (int k = 0; k < EV; ++k)
@@ -750,22 +775,29 @@ void launch_rs(const RSParams& p, int grid, cudaStream_t s) {
   check_launch("rs_kernel");
 }
 
-template <typename T, bool MC, bool ADAM, bool CLIP>
+template <typename T, bool MC, int OPT, bool CLIP>
 static void launch_ag_wa(const AGParams& p, int grid, cudaStream_t s) {
   switch (p.world) {
-    case 1: ag_kernel<T, 1, MC, ADAM, CLIP><<<grid, kThreads, 0, s>>>(p); break;
-    case 2: ag_kernel<T, 2, MC, ADAM, CLIP><<<grid, kThreads, 0, s>>>(p); break;
-    case 4: ag_kernel<T, 4, MC, ADAM, CLIP><<<grid, kThreads, 0, s>>>(p); break;
-    case 8: ag_kernel<T, 8, MC, ADAM, CLIP><<<grid, kThreads, 0, s>>>(p); break;
-    default: ag_kernel<T, 0, MC, ADAM, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    case 1: ag_kernel<T, 1, MC, OPT, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    case 2: ag_kernel<T, 2, MC, OPT, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    case 4: ag_kernel<T, 4, MC, OPT, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    case 8: ag_kernel<T, 8, MC, OPT, CLIP><<<grid, kThreads, 0, s>>>(p); break;
+    default: ag_kernel<T, 0, MC, OPT, CLIP><<<grid, kThreads, 0, s>>>(p); break;
   }
+}
+
+template <typename T, bool MC, int OPT>
+static void launch_ag_wo(const AGParams& p, int grid, cudaStream_t s) {
+  if (p.clip != nullptr && p.do_update) launch_ag_wa<T, MC, OPT, true>(p, grid, s);
+  else launch_ag_wa<T, MC, OPT, false>(p, grid, s);
 }
 
 template <typename T, bool MC>
 static void launch_ag_w(const AGParams& p, int grid, cudaStream_t s) {
-  const bool adam = p.adam && p.do_update, clip = p.clip != nullptr && p.do_update;
-  if (adam) clip ? launch_ag_wa<T, MC, true, true>(p, grid, s) : launch_ag_wa<T, MC, true, false>(p, grid, s);
-  else clip ? launch_ag_wa<T, MC, false, true>(p, grid, s) : launch_ag_wa<T, MC, false, false>(p, grid, s);
+  // a pure all-gather (no update) runs the SGD instantiation, whatever the optimizer
+  if (p.do_update && p.adam) launch_ag_wo<T, MC, AG_ADAM>(p, grid, s);
+  else if (p.do_update && p.rmsprop) launch_ag_wo<T, MC, AG_RMSPROP>(p, grid, s);
+  else launch_ag_wo<T, MC, AG_SGD>(p, grid, s);
 }
 
 void launch_ag(const AGParams& p, int grid, cudaStream_t s) {

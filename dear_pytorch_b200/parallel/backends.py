@@ -28,13 +28,15 @@ from .bucket import BucketPlan
 _DT_CODE = {torch.float32: "DT_F32", torch.bfloat16: "DT_BF16", torch.float16: "DT_F16"}
 
 
-OPT_SGD, OPT_ADAM, OPT_ADAMW = 0, 1, 2
-HYPER_NESTEROV, HYPER_SKIP = 1, 2        # bits of the ``nesterov`` field of a hyper segment (csrc/dear_common.h)
+OPT_SGD, OPT_ADAM, OPT_ADAMW, OPT_RMSPROP = 0, 1, 2, 3
+HYPER_NESTEROV, HYPER_SKIP, HYPER_CENTERED = 1, 2, 4   # bits of the ``nesterov`` field of a hyper segment (csrc/dear_common.h)
 
 
 class HyperSpec:
     """Per-bucket hyper-parameter segments:
-    ``[(end_elem, lr, wd, momentum|beta1, dampening, nesterov, opt, beta2, eps)]`` (opt: 0 SGD, 1 Adam, 2 AdamW)."""
+    ``[(end_elem, lr, wd, momentum|beta1, dampening, nesterov, opt, beta2, eps)]`` (opt: 0 SGD, 1 Adam, 2 AdamW,
+    3 RMSprop).  RMSprop stores ``1 - alpha`` in ``dampening``, ``alpha`` in ``beta2`` and ``centered`` as the
+    HYPER_CENTERED bit of ``nesterov``."""
 
     __slots__ = ("segs",)
 
@@ -46,11 +48,26 @@ class HyperSpec:
 
     @property
     def is_adam(self):
-        return any(s[6] != OPT_SGD for s in self.segs)
+        return any(s[6] in (OPT_ADAM, OPT_ADAMW) for s in self.segs)
+
+    @property
+    def is_rmsprop(self):
+        return any(s[6] == OPT_RMSPROP for s in self.segs)
 
     @property
     def uses_momentum(self):
+        """Needs a momentum shard: Adam's exp_avg, or an SGD / RMSprop momentum buffer (momentum > 0)."""
         return self.is_adam or any(s[3] > 0 for s in self.segs)
+
+    @property
+    def uses_var(self):
+        """Needs a second-moment shard: Adam's exp_avg_sq or RMSprop's square_avg."""
+        return self.is_adam or self.is_rmsprop
+
+    @property
+    def uses_grad_avg(self):
+        """Needs a grad_avg shard: some RMSprop segment is centered."""
+        return any(s[6] == OPT_RMSPROP and int(s[5]) & HYPER_CENTERED for s in self.segs)
 
 
 class _BackendBase:
@@ -68,7 +85,8 @@ class _BackendBase:
         self.grad_shard: List[torch.Tensor] = [None] * nb
         self.mom_shard: List[Optional[torch.Tensor]] = [None] * nb
         self.master_shard: List[Optional[torch.Tensor]] = [None] * nb
-        self.var_shard: List[Optional[torch.Tensor]] = [None] * nb       # Adam exp_avg_sq
+        self.var_shard: List[Optional[torch.Tensor]] = [None] * nb       # Adam exp_avg_sq / RMSprop square_avg
+        self.gavg_shard: List[Optional[torch.Tensor]] = [None] * nb      # centered RMSprop grad_avg
         self.hyper: List[Optional[HyperSpec]] = [None] * nb
         self.grad_scale = 1.0
         self.amp: Optional[torch.Tensor] = None     # dynamic loss scaler state (parallel/grad_scaler.py), engine-owned
@@ -96,6 +114,20 @@ class _BackendBase:
         if self.var_shard[g] is None:
             self.var_shard[g] = torch.zeros(self.plan.buckets[g].shard_numel, dtype=torch.float32, device=self.device)
             self._shards_changed(g)
+
+    def ensure_grad_avg(self, g: int):
+        if self.gavg_shard[g] is None:
+            self.gavg_shard[g] = torch.zeros(self.plan.buckets[g].shard_numel, dtype=torch.float32, device=self.device)
+            self._shards_changed(g)
+
+    def _ensure_state(self, g: int, spec: "HyperSpec"):
+        """Allocate (zeroed) the state shards the optimizer of ``spec`` reads."""
+        if spec.uses_momentum:
+            self.ensure_momentum(g)
+        if spec.uses_var:
+            self.ensure_var(g)
+        if spec.uses_grad_avg:
+            self.ensure_grad_avg(g)
 
     def _shards_changed(self, g: Optional[int] = None):
         pass
@@ -180,16 +212,14 @@ class NativeBackend(_BackendBase):
         for i in (range(len(self.where)) if g is None else (g,)):
             bs, li = self.where[i]
             if self.grad_shard[i] is not None:
-                bs.set_shards(li, self.grad_shard[i], self.mom_shard[i], self.master_shard[i], self.var_shard[i])
+                bs.set_shards(li, self.grad_shard[i], self.mom_shard[i], self.master_shard[i], self.var_shard[i],
+                              self.gavg_shard[i])
 
     def set_hyper(self, g, spec: HyperSpec):
         if self.hyper[g] == spec:
             return
         self.hyper[g] = spec
-        if spec.uses_momentum:
-            self.ensure_momentum(g)
-        if spec.is_adam:
-            self.ensure_var(g)
+        self._ensure_state(g, spec)
         bs, li = self.where[g]
         bs.set_hyper(li, [s[0] for s in spec.segs], [s[1] for s in spec.segs], [s[2] for s in spec.segs],
                      [s[3] for s in spec.segs], [s[4] for s in spec.segs], [int(s[5]) for s in spec.segs],
@@ -293,10 +323,7 @@ class TorchBackend(_BackendBase):
 
     def set_hyper(self, g, spec: HyperSpec):
         self.hyper[g] = spec
-        if spec.uses_momentum:
-            self.ensure_momentum(g)
-        if spec.is_adam:
-            self.ensure_var(g)
+        self._ensure_state(g, spec)
 
     def set_step(self, t: int):
         self._t = int(t)
@@ -381,12 +408,33 @@ class TorchBackend(_BackendBase):
                 continue
             if int(nesterov) & HYPER_SKIP and not bool(self.grad_shard[g][a - lo:z - lo].any()):
                 continue                          # no gradient on ANY rank this step: parameter and state stay as they are
+            centered = bool(int(nesterov) & HYPER_CENTERED)
             nesterov = bool(int(nesterov) & HYPER_NESTEROV)
             sl = slice(a - lo, z - lo)
             p = master[sl] if master is not None else self._pbuf[g][a:z]
             d = self.grad_shard[g][sl]
             if self.clip is not None:
                 d = d * self.clip[2]
+            if opt == OPT_RMSPROP:
+                # torch.optim.RMSprop (_single_tensor_rmsprop); alpha is beta2, 1 - alpha is damp
+                if wd != 0:
+                    d = d.add(p, alpha=wd)
+                sq = self.var_shard[g][sl]
+                sq.mul_(beta2).addcmul_(d, d, value=damp)
+                if centered:
+                    ga = self.gavg_shard[g][sl]
+                    ga.lerp_(d, damp)
+                    avg = sq.addcmul(ga, ga, value=-1).sqrt_().add_(eps)
+                else:
+                    avg = sq.sqrt().add_(eps)
+                if mom > 0:
+                    buf = self.mom_shard[g][sl]
+                    buf.mul_(mom).addcdiv_(d, avg)
+                    p.add_(buf, alpha=-lr)
+                else:
+                    p.addcdiv_(d, avg, value=-lr)
+                self._n_launch += 5
+                continue
             if opt != OPT_SGD:
                 t = self._t + 1
                 m, v = self.mom_shard[g][sl], self.var_shard[g][sl]

@@ -32,7 +32,8 @@ import torch
 import torch.nn as nn
 
 from .. import runtime
-from .backends import HYPER_SKIP, OPT_ADAM, OPT_ADAMW, OPT_SGD, HyperSpec, NativeBackend, TorchBackend
+from .backends import (HYPER_CENTERED, HYPER_SKIP, OPT_ADAM, OPT_ADAMW, OPT_RMSPROP, OPT_SGD, HyperSpec, NativeBackend,
+                       TorchBackend)
 from .bucket import BucketPlan
 
 import weakref
@@ -90,6 +91,8 @@ class DearEngine:
             self.opt_kind = OPT_ADAMW
         elif isinstance(optimizer, torch.optim.Adam):
             self.opt_kind = OPT_ADAM
+        elif isinstance(optimizer, torch.optim.RMSprop):
+            self.opt_kind = OPT_RMSPROP
         else:
             self.opt_kind = OPT_SGD
         self._hooks = []
@@ -101,9 +104,10 @@ class DearEngine:
         for p in model.parameters():
             if p.requires_grad and p.device.type != self.device.type:
                 raise RuntimeError("model parameters live on %s but the runtime device is %s" % (p.device, self.device))
-        # Adam / AdamW: updates a parameter did NOT take part in (no gradient on any rank).  torch.optim keeps the step
-        # count per parameter, the kernels keep one per bucket set: _refresh_hyper folds the difference into the
-        # parameter's hyper segment (see _adam_lag_adjust)
+        # Adam / AdamW / RMSprop: updates a parameter did NOT take part in (no gradient on any rank).  torch.optim keeps
+        # the step count per parameter, the kernels keep one per bucket set: for Adam _refresh_hyper folds the difference
+        # into the parameter's hyper segment (see _adam_lag_adjust); RMSprop's math does not depend on the count, which
+        # only appears in its state_dict()
         self._lag: Dict[nn.Parameter, int] = {}
         # SGD with momentum AND dampening: torch initialises a parameter's momentum buffer with its first gradient
         # (undampened); the kernels know one global "first step".  Parameters that start later get dampening 0 in
@@ -383,7 +387,7 @@ class DearEngine:
         for b in self.plan.buckets:
             absent = self._absent[b.index]
             lags = None
-            if self.opt_kind != OPT_SGD and self._lag:
+            if self.opt_kind in (OPT_ADAM, OPT_ADAMW) and self._lag:
                 # (a parameter that sits this step out as well needs no correction now: no table churn for a branch
                 # that never runs)
                 gone_now = set(absent)
@@ -491,12 +495,19 @@ class DearEngine:
         return frozen if frozen is not None else self._hyper_key_live()
 
     def _hyper_key_live(self):
-        """Per param group: (lr, wd, momentum|beta1, dampening, nesterov, opt, beta2, eps)."""
+        """Per param group: (lr, wd, momentum|beta1, dampening, nesterov, opt, beta2, eps).  RMSprop: (lr, wd,
+        momentum, 1 - alpha, HYPER_CENTERED if centered, OPT_RMSPROP, alpha, eps)."""
         keys = []
         for g in self.opt.param_groups:
             if self.opt_kind == OPT_SGD:
                 keys.append((float(g["lr"]), float(g.get("weight_decay", 0.0)), float(g.get("momentum", 0.0)),
                              float(g.get("dampening", 0.0)), bool(g.get("nesterov", False)), OPT_SGD, 0.0, 0.0))
+            elif self.opt_kind == OPT_RMSPROP:
+                alpha = float(g["alpha"])
+                # 1 - alpha is formed in double and rounded once, like the Python scalar torch hands to its kernels
+                keys.append((float(g["lr"]), float(g.get("weight_decay", 0.0)), float(g.get("momentum", 0.0)),
+                             1.0 - alpha, HYPER_CENTERED if g.get("centered", False) else 0, OPT_RMSPROP, alpha,
+                             float(g["eps"])))
             else:
                 b1, b2 = g["betas"]
                 keys.append((float(g["lr"]), float(g.get("weight_decay", 0.0)), float(b1), 0.0, False, self.opt_kind,
@@ -694,7 +705,8 @@ class DearEngine:
     def _gather_state(self) -> dict:
         """Full (un-sharded) optimizer state per parameter name: momentum and fp32 master."""
         from ..utils.checkpoint import gather_sharded
-        out = {"momentum": {}, "master": {}, "var": {}, "mom_init": self._mom_initialised, "num_updates": self.num_updates}
+        out = {"momentum": {}, "master": {}, "var": {}, "gavg": {}, "mom_init": self._mom_initialised,
+               "num_updates": self.num_updates}
         if self.amp is not None:
             # skipped steps applied nothing: the device count of applied updates is the step count of the new buckets
             applied = self.read_scaler()["applied"]
@@ -702,7 +714,7 @@ class DearEngine:
         for b in self.plan.buckets:
             g = b.index
             for kind, shard in (("momentum", self.backend.mom_shard[g]), ("master", self.backend.master_shard[g]),
-                                ("var", self.backend.var_shard[g])):
+                                ("var", self.backend.var_shard[g]), ("gavg", self.backend.gavg_shard[g])):
                 if shard is None:
                     continue
                 full = gather_sharded(shard, self.world)
@@ -719,7 +731,7 @@ class DearEngine:
         for b in self.plan.buckets:
             g = b.index
             lo, hi = self.rank * b.shard_numel, (self.rank + 1) * b.shard_numel
-            for kind in ("momentum", "master", "var"):
+            for kind in ("momentum", "master", "var", "gavg"):
                 vals = carry.get(kind, {})
                 if not any(s.name in vals for s in b.slots):
                     continue
@@ -729,6 +741,9 @@ class DearEngine:
                 elif kind == "var":
                     be.ensure_var(g)
                     shard = be.var_shard[g]
+                elif kind == "gavg":
+                    be.ensure_grad_avg(g)
+                    shard = be.gavg_shard[g]
                 else:
                     shard = be.master_shard[g]
                     if shard is None:
@@ -783,11 +798,18 @@ class _DistributedOptimizer(torch.optim.Optimizer):
     def __init__(self, params, model, threshold=THRESHOLD, num_nearby_layers=NUM_NEARBY_LAYERS,
                  exclude_parts="", policy=None, verbose=True, backward_passes_per_step=1, grad_comm_dtype=None):
         super(self.__class__, self).__init__(params)
-        if not isinstance(self, (torch.optim.SGD, torch.optim.Adam, torch.optim.AdamW)):
+        if not isinstance(self, (torch.optim.SGD, torch.optim.Adam, torch.optim.AdamW, torch.optim.RMSprop)):
             raise TypeError(
                 "the decoupled all-reduce fuses the parameter update into the all-gather kernel; supported: "
-                "torch.optim.SGD (the reference's only DeAR optimizer, dear/dear_dopt.py:310-336), Adam and AdamW; "
-                "got %s. Use parallel.baselines for other optimizers." % type(self).__mro__[1].__name__)
+                "torch.optim.SGD (the reference's only DeAR optimizer, dear/dear_dopt.py:310-336), Adam, AdamW and "
+                "RMSprop; got %s. Use parallel.baselines for other optimizers." % type(self).__mro__[1].__name__)
+        if isinstance(self, torch.optim.RMSprop):
+            for g in self.param_groups:
+                for k in ("maximize", "capturable", "differentiable"):
+                    if g.get(k, False):
+                        raise ValueError("RMSprop with %s=True is not supported by the fused update" % k)
+                if isinstance(g["lr"], torch.Tensor):
+                    raise ValueError("RMSprop with a tensor lr is not supported by the fused update (pass a float)")
         for g in self.param_groups:
             if g.get("amsgrad", False) or g.get("capturable", False) or g.get("differentiable", False):
                 raise ValueError("amsgrad / capturable / differentiable Adam variants are not supported")
@@ -846,7 +868,10 @@ def DistributedOptimizer(optimizer, model, compression=None, is_sparse=False, de
                          fp16=False, mgwfbp=False, rdma=False, multi_job_scheduling=False, exclude_parts="",
                          num_nearby_layers=None, policy=None, verbose=True, bo_tuning=False, bo_kwargs=None,
                          backward_passes_per_step=1, loss_scale=None, grad_comm_dtype=None):
-    """Wrap ``optimizer`` (``torch.optim.SGD`` / ``Adam`` / ``AdamW``) for DeAR data-parallel training of ``model``.
+    """Wrap ``optimizer`` (``torch.optim.SGD`` / ``Adam`` / ``AdamW`` / ``RMSprop``) for DeAR data-parallel training of
+    ``model``.  RMSprop runs with every option of its parameter groups (``alpha``, ``eps``, ``weight_decay``,
+    ``momentum``, ``centered``), inside the same fused update kernel; ``maximize``, ``capturable``, ``differentiable``
+    and a tensor ``lr`` raise ``ValueError``.
 
     Signature-compatible with the reference factory (dear/dear_dopt.py:381-398): the Horovod-era
     keyword arguments are accepted; those that have no meaning here are ignored.  Unlike the

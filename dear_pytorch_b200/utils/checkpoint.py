@@ -5,9 +5,10 @@ weights sharded 1/P per rank (Kernel B) a checkpoint has to gather the shards, a
 to scatter them — possibly into a *different* bucket layout or world size.  State is therefore
 exchanged per parameter *name*, never per bucket.
 
-``optimizer.state_dict()`` (collective) returns a ``torch.optim.SGD``-compatible dict — the full
-``momentum_buffer`` per parameter — so a checkpoint written by DeAR loads into stock PyTorch and
-vice versa.
+``optimizer.state_dict()`` (collective) returns a dict in the layout of the wrapped ``torch.optim`` class — the full
+``momentum_buffer`` per parameter for SGD, ``step`` / ``exp_avg`` / ``exp_avg_sq`` for Adam and AdamW, ``step`` /
+``square_avg`` (+ ``momentum_buffer`` with momentum, + ``grad_avg`` when centered) for RMSprop — so a checkpoint written
+by DeAR loads into stock PyTorch and vice versa.
 """
 from __future__ import annotations
 
@@ -18,6 +19,7 @@ import torch
 import torch.distributed as dist
 
 from .. import runtime
+from ..parallel.backends import OPT_ADAM, OPT_ADAMW, OPT_RMSPROP, OPT_SGD
 
 
 @torch.no_grad()
@@ -53,7 +55,19 @@ def optimizer_state_dict(optimizer) -> dict:
     state = {}
     for s in eng.plan.slots:
         ent = {}
-        if eng.opt_kind != 0:              # Adam / AdamW: torch.optim.Adam state layout
+        if eng.opt_kind == OPT_RMSPROP:
+            # torch.optim.RMSprop layout: no entry before a parameter's first gradient; momentum_buffer / grad_avg only
+            # in groups that have momentum / are centered
+            steps = carry["num_updates"] - eng._lag.get(s.param, 0)
+            if steps > 0 and s.name in carry["var"]:
+                grp = optimizer.param_groups[eng.group_of[s.param]]
+                ent["step"] = torch.tensor(float(steps))
+                ent["square_avg"] = carry["var"][s.name].reshape(s.param.shape).clone()
+                if grp["momentum"] > 0:
+                    ent["momentum_buffer"] = carry["momentum"][s.name].reshape(s.param.shape).clone()
+                if grp["centered"]:
+                    ent["grad_avg"] = carry["gavg"][s.name].reshape(s.param.shape).clone()
+        elif eng.opt_kind in (OPT_ADAM, OPT_ADAMW):   # torch.optim.Adam state layout
             if s.name in carry["momentum"]:
                 # torch.optim.Adam counts steps per parameter: updates this one sat out (no gradient) are not counted
                 ent["step"] = torch.tensor(float(carry["num_updates"] - eng._lag.get(s.param, 0)))
@@ -78,7 +92,7 @@ def optimizer_state_dict(optimizer) -> dict:
 
 @torch.no_grad()
 def load_optimizer_state_dict(optimizer, sd: dict) -> None:
-    """Collective.  Accepts a dict from ``optimizer_state_dict`` or from a stock ``torch.optim.SGD``."""
+    """Collective.  Accepts a dict from ``optimizer_state_dict`` or from the stock ``torch.optim`` class."""
     eng = optimizer._dear
     eng.flush()
     for g, saved in zip(optimizer.param_groups, sd["param_groups"]):
@@ -87,10 +101,10 @@ def load_optimizer_state_dict(optimizer, sd: dict) -> None:
                 g[k] = v
     index = _param_index(optimizer)
     meta = sd.get("dear") or {}
-    carry = {"momentum": {}, "master": {}, "var": {}, "mom_init": False,
+    carry = {"momentum": {}, "master": {}, "var": {}, "gavg": {}, "mom_init": False,
              "num_updates": int(meta.get("num_updates", eng.num_updates))}
     adam_steps = {}
-    track_first = eng.opt_kind == 0 and any(g.get("momentum", 0) != 0 and g.get("dampening", 0) != 0
+    track_first = eng.opt_kind == OPT_SGD and any(g.get("momentum", 0) != 0 and g.get("dampening", 0) != 0
                                             for g in optimizer.param_groups)
     eng._virgin = {s.param for s in eng.plan.slots} if track_first else set()
     for s in eng.plan.slots:
@@ -109,6 +123,11 @@ def load_optimizer_state_dict(optimizer, sd: dict) -> None:
             carry["var"][s.name] = ent["exp_avg_sq"].to(eng.device, torch.float32).reshape(-1)
             if ent.get("step") is not None:
                 adam_steps[s.param] = int(float(ent["step"]))
+        if ent.get("square_avg") is not None:
+            carry["var"][s.name] = ent["square_avg"].to(eng.device, torch.float32).reshape(-1)
+            if ent.get("grad_avg") is not None:
+                carry["gavg"][s.name] = ent["grad_avg"].to(eng.device, torch.float32).reshape(-1)
+            adam_steps[s.param] = int(float(ent["step"]))
         mp = ent.get("master_param")
         if mp is not None:
             carry["master"][s.name] = mp.to(eng.device, torch.float32).reshape(-1)
@@ -117,7 +136,13 @@ def load_optimizer_state_dict(optimizer, sd: dict) -> None:
         # through their hyper segment (DearEngine._adam_lag_adjust)
         carry["num_updates"] = max(adam_steps.values())
         eng._lag = {p: carry["num_updates"] - v for p, v in adam_steps.items() if v < carry["num_updates"]}
-    if eng.opt_kind == 0 and carry["mom_init"]:
+        if eng.opt_kind == OPT_RMSPROP:
+            # a parameter without an entry has not had a gradient yet (its state is zero, and so is its count)
+            eng._lag.update({s.param: carry["num_updates"] for s in eng.plan.slots if s.param not in adam_steps})
+    elif eng.opt_kind == OPT_RMSPROP:
+        carry["num_updates"] = 0           # no parameter has state: nothing has been applied yet
+        eng._lag = {}
+    if eng.opt_kind == OPT_SGD and carry["mom_init"]:
         # momentum buffers exist, so the next update is not the first one (a stock torch.optim.SGD state has no count)
         carry["num_updates"] = max(carry["num_updates"], 1)
     eng._restore_state(carry)

@@ -3,16 +3,21 @@
 
     torchrun --nproc-per-node N tools/kernel_bench.py [--sizes-mb 1,4,16,24,64,392] [--dtype fp32]
                                                       [--grad-comm-dtype fp32|bf16|fp16]
+                                                      [--optimizer sgd|adam|rmsprop|rmsprop-centered]
 
 For every bucket size it times (CUDA events, after warm-up, max over ranks)
   Kernel A  rs_kernel : pack + reduce-scatter + fp32 accumulate + 1/P scale
-  Kernel B  ag_kernel : sharded SGD(momentum) + all-gather push
+  Kernel B  ag_kernel : sharded update (--optimizer: SGD with momentum, Adam, RMSprop with momentum, centered RMSprop
+                        with momentum) + all-gather push
 and the NCCL collectives the reference issues for the same bucket
 (reduce_scatter_tensor / all_gather_into_tensor, without the reference's extra elementwise kernels).
 Bus bandwidth = bytes * (P-1)/P / time, reported against the H100 SXM data sheet's 450 GB/s per direction
 (utils/perf_model.py); at P = 1 the HBM roofline applies instead.  ``--grad-comm-dtype bf16|fp16`` (fp32 buckets, P > 1)
 sends the gradients at 16 bits: the pack reads fp32 and writes 16-bit wire elements, the pull reads wire bytes.
-``rs_link_bytes`` / ``rs_hbm_bytes`` are the byte model of Kernel A per rank.  With ranks sharing one GPU, "peer" loads
+``rs_link_bytes`` / ``rs_hbm_bytes`` are the byte model of Kernel A per rank; ``ag_hbm_read_bytes`` / ``ag_hbm_write_bytes``
+that of Kernel B (parameter or fp32 master, gradient shard and optimizer state read; state, master and the pushed
+parameter copies written), and ``ag_hbm_gbs`` / ``ag_frac_of_hbm`` the achieved rate against 3.35 TB/s (H100 SXM data
+sheet) — meaningful at P = 1, where every byte is local.  With ranks sharing one GPU, "peer" loads
 read local HBM, so those times say nothing about the link.
 """
 import argparse
@@ -31,12 +36,26 @@ from dear_pytorch_b200 import ops  # noqa: E402
 from dear_pytorch_b200.utils import perf_model  # noqa: E402
 
 
+# Kernel B's hyper row (set_hyper keywords) and fp32 state arrays per optimizer
+OPTIMIZERS = {
+    "sgd": (dict(weight_decay=[1e-4], momentum=[0.9], dampening=[0.0], nesterov=[0]), ("momentum",)),
+    "adam": (dict(weight_decay=[0.0], momentum=[0.9], dampening=[0.0], nesterov=[0], opt=[1], beta2=[0.999],
+                  eps=[1e-8]), ("momentum", "var")),
+    "rmsprop": (dict(weight_decay=[0.0], momentum=[0.9], dampening=[1.0 - 0.99], nesterov=[0], opt=[3], beta2=[0.99],
+                     eps=[1e-8]), ("momentum", "var")),
+    "rmsprop-centered": (dict(weight_decay=[0.0], momentum=[0.9], dampening=[1.0 - 0.99], nesterov=[4], opt=[3],
+                              beta2=[0.99], eps=[1e-8]), ("momentum", "var", "grad_avg")),
+}
+HBM_TBS = 3.35                                   # H100 SXM HBM3 data sheet
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sizes-mb", default="1,4,16,24,64,392")
     ap.add_argument("--dtype", default="fp32", choices=["fp32", "bf16"])
     ap.add_argument("--grad-comm-dtype", default="fp32", choices=["fp32", "bf16", "fp16"],
                     help="--dtype fp32 only: dtype of the gradient buckets (the pack rounds the fp32 gradients)")
+    ap.add_argument("--optimizer", default="sgd", choices=sorted(OPTIMIZERS))
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--nccl", type=int, default=1)
     ap.add_argument("--out", default=None)
@@ -86,19 +105,30 @@ def main():
         shard = n // world
         grad_src = torch.randn(n, device=dev).to(tdt)                   # "autograd output" to be packed
         gs = torch.zeros(shard, device=dev)
-        mom = torch.zeros(shard, device=dev)
+        hyper, state = OPTIMIZERS[args.optimizer]
+        sh = {k: torch.zeros(shard, device=dev) for k in state}
         master = torch.zeros(shard, device=dev) if args.dtype != "fp32" else None
-        bs.set_shards(g, gs, mom, master)
+        bs.set_shards(g, gs, sh.get("momentum"), master, sh.get("var"), sh.get("grad_avg"))
         bs.set_pack(g, [grad_src.data_ptr()], [0], [wbytes], [0])
-        bs.set_hyper(g, [n], [0.01], [1e-4], [0.9], [0.0], [0])
+        bs.set_hyper(g, [n], [0.01], **hyper)
         bs.param_buffer(g).normal_()
         torch.cuda.synchronize()
         t_rs = timed(lambda: bs.reduce_scatter(g, True), args.iters)
         t_rs_nopack = timed(lambda: bs.reduce_scatter(g, False), args.iters)
         t_ag = timed(lambda: bs.allgather_update(g, True, False, True, False), args.iters)
+        opt_key = args.optimizer.replace("-", "_")
         row = {"bucket_mb": round(nbytes / 2 ** 20, 2), "dtype": args.dtype, "grad_comm_dtype": wire or args.dtype,
-               "world": world, "rs_plan": bs.rs_plan(g),
-               "rs_us": round(t_rs, 2), "rs_nopack_us": round(t_rs_nopack, 2), "ag_sgd_us": round(t_ag, 2)}
+               "world": world, "optimizer": args.optimizer, "rs_plan": bs.rs_plan(g),
+               "rs_us": round(t_rs, 2), "rs_nopack_us": round(t_rs_nopack, 2), "ag_%s_us" % opt_key: round(t_ag, 2)}
+        # Kernel B per rank: reads the parameter shard (or its fp32 master), the gradient shard and every state array;
+        # writes the state arrays (and master) and one copy of the parameter shard per rank
+        n_state = len(state)
+        p_bytes = 4 if master is not None else es
+        ag_rd = shard * (p_bytes + 4 + 4 * n_state)
+        ag_wr = shard * (4 * n_state + (4 if master is not None else 0) + es * world)
+        row["ag_hbm_read_bytes"], row["ag_hbm_write_bytes"] = int(ag_rd), int(ag_wr)
+        row["ag_hbm_gbs"] = round((ag_rd + ag_wr) / t_ag / 1e3, 1)
+        row["ag_frac_of_hbm"] = round((ag_rd + ag_wr) / t_ag / 1e6 / HBM_TBS, 3)
         rr = perf_model.rs_roofline_us(wbytes, world, wes, peaks, src_elem_bytes=es)
         row["rs_link_bytes"] = int(rr["link_bytes"])
         row["rs_hbm_bytes"] = int(rr["hbm_bytes"])
