@@ -5,14 +5,15 @@
                    elementwise kernel on either the backward or the forward path.
 ``TorchBackend``   (nccl / gloo): the same bucket layout driven by
                    ``torch.distributed.reduce_scatter_tensor`` / ``all_gather_into_tensor`` and
-                   an eager sharded SGD — the comparison baseline and the CPU plumbing path.
-                   This is what the reference does per bucket (dear/tensorfusion.py:469-482,
-                   dear/dear_dopt.py:293-336), minus its per-parameter loops.
+                   the optimizer family's eager sharded update (parallel/families.py) — the
+                   comparison baseline and the CPU plumbing path.  This is what the reference
+                   does per bucket (dear/tensorfusion.py:469-482, dear/dear_dopt.py:293-336),
+                   minus its per-parameter loops.
 
 Both expose the same interface to ``parallel.optimizer``:
   param_buffer(g) / grad_buffer(g)      flat bucket tensors (parameters / gradients are views)
   reduce_scatter(g, pack)               backward-path collective (+ 1/P scale)
-  allgather_update(g, ...)              forward-path collective (+ sharded SGD)
+  allgather_update(g, ...)              forward-path collective (+ sharded update)
   wait_bucket(g) / wait_all() / fence() / synchronize()
 """
 from __future__ import annotations
@@ -24,57 +25,18 @@ import torch.distributed as dist
 
 from .. import ops
 from .bucket import BucketPlan
+from .families import HYPER_SKIP, HyperRow
 
 _DT_CODE = {torch.float32: "DT_F32", torch.bfloat16: "DT_BF16", torch.float16: "DT_F16"}
-
-
-OPT_SGD, OPT_ADAM, OPT_ADAMW, OPT_RMSPROP = 0, 1, 2, 3
-HYPER_NESTEROV, HYPER_SKIP, HYPER_CENTERED = 1, 2, 4   # bits of the ``nesterov`` field of a hyper segment (csrc/dear_common.h)
-
-
-class HyperSpec:
-    """Per-bucket hyper-parameter segments:
-    ``[(end_elem, lr, wd, momentum|beta1, dampening, nesterov, opt, beta2, eps)]`` (opt: 0 SGD, 1 Adam, 2 AdamW,
-    3 RMSprop).  RMSprop stores ``1 - alpha`` in ``dampening``, ``alpha`` in ``beta2`` and ``centered`` as the
-    HYPER_CENTERED bit of ``nesterov``."""
-
-    __slots__ = ("segs",)
-
-    def __init__(self, segs):
-        self.segs = tuple(tuple(s) + (OPT_SGD, 0.0, 0.0)[len(s) - 6:] if len(s) < 9 else tuple(s) for s in segs)
-
-    def __eq__(self, other):
-        return isinstance(other, HyperSpec) and self.segs == other.segs
-
-    @property
-    def is_adam(self):
-        return any(s[6] in (OPT_ADAM, OPT_ADAMW) for s in self.segs)
-
-    @property
-    def is_rmsprop(self):
-        return any(s[6] == OPT_RMSPROP for s in self.segs)
-
-    @property
-    def uses_momentum(self):
-        """Needs a momentum shard: Adam's exp_avg, or an SGD / RMSprop momentum buffer (momentum > 0)."""
-        return self.is_adam or any(s[3] > 0 for s in self.segs)
-
-    @property
-    def uses_var(self):
-        """Needs a second-moment shard: Adam's exp_avg_sq or RMSprop's square_avg."""
-        return self.is_adam or self.is_rmsprop
-
-    @property
-    def uses_grad_avg(self):
-        """Needs a grad_avg shard: some RMSprop segment is centered."""
-        return any(s[6] == OPT_RMSPROP and int(s[5]) & HYPER_CENTERED for s in self.segs)
+SHARD_KINDS = ("mom", "var", "gavg", "master")    # a bucket's fp32 shards: family state (parallel/families.py), master
 
 
 class _BackendBase:
     steal_grads = False
 
-    def __init__(self, plan: BucketPlan, rank: int, world: int, device: torch.device,
+    def __init__(self, family, plan: BucketPlan, rank: int, world: int, device: torch.device,
                  grad_comm_dtype: Optional[torch.dtype] = None):
+        self.family = family            # parallel/families.py: which state shards a bucket needs, the eager update
         self.plan = plan
         self.rank = rank
         self.world = world
@@ -83,11 +45,8 @@ class _BackendBase:
         self.wire = grad_comm_dtype if world > 1 else None
         nb = len(plan.buckets)
         self.grad_shard: List[torch.Tensor] = [None] * nb
-        self.mom_shard: List[Optional[torch.Tensor]] = [None] * nb
-        self.master_shard: List[Optional[torch.Tensor]] = [None] * nb
-        self.var_shard: List[Optional[torch.Tensor]] = [None] * nb       # Adam exp_avg_sq / RMSprop square_avg
-        self.gavg_shard: List[Optional[torch.Tensor]] = [None] * nb      # centered RMSprop grad_avg
-        self.hyper: List[Optional[HyperSpec]] = [None] * nb
+        self.shards: List[Dict[str, torch.Tensor]] = [{} for _ in range(nb)]     # per bucket: kind -> fp32 shard
+        self.hyper: List[Optional[Tuple[HyperRow, ...]]] = [None] * nb
         self.grad_scale = 1.0
         self.amp: Optional[torch.Tensor] = None     # dynamic loss scaler state (parallel/grad_scaler.py), engine-owned
         self.clip: Optional[torch.Tensor] = None    # global-norm clipping state (ClipState, csrc/dear_common.h), engine-owned
@@ -102,32 +61,17 @@ class _BackendBase:
         for b in self.plan.buckets:
             if b.dtype != torch.float32:
                 lo = self.rank * b.shard_numel
-                self.master_shard[b.index] = self.param_buffer(b.index)[lo:lo + b.shard_numel].float().clone()
+                self.shards[b.index]["master"] = self.param_buffer(b.index)[lo:lo + b.shard_numel].float().clone()
         self._shards_changed()
 
-    def ensure_momentum(self, g: int):
-        if self.mom_shard[g] is None:
-            self.mom_shard[g] = torch.zeros(self.plan.buckets[g].shard_numel, dtype=torch.float32, device=self.device)
+    def ensure_state(self, g: int, kind: str) -> torch.Tensor:
+        """The ``kind`` state shard of bucket g, allocated (zeroed) on first use."""
+        shard = self.shards[g].get(kind)
+        if shard is None:
+            shard = self.shards[g][kind] = torch.zeros(self.plan.buckets[g].shard_numel, dtype=torch.float32,
+                                                       device=self.device)
             self._shards_changed(g)
-
-    def ensure_var(self, g: int):
-        if self.var_shard[g] is None:
-            self.var_shard[g] = torch.zeros(self.plan.buckets[g].shard_numel, dtype=torch.float32, device=self.device)
-            self._shards_changed(g)
-
-    def ensure_grad_avg(self, g: int):
-        if self.gavg_shard[g] is None:
-            self.gavg_shard[g] = torch.zeros(self.plan.buckets[g].shard_numel, dtype=torch.float32, device=self.device)
-            self._shards_changed(g)
-
-    def _ensure_state(self, g: int, spec: "HyperSpec"):
-        """Allocate (zeroed) the state shards the optimizer of ``spec`` reads."""
-        if spec.uses_momentum:
-            self.ensure_momentum(g)
-        if spec.uses_var:
-            self.ensure_var(g)
-        if spec.uses_grad_avg:
-            self.ensure_grad_avg(g)
+        return shard
 
     def _shards_changed(self, g: Optional[int] = None):
         pass
@@ -136,8 +80,11 @@ class _BackendBase:
         """Number of updates already applied (Adam bias correction); called after (re)building buckets."""
         pass
 
-    def set_hyper(self, g: int, spec: HyperSpec) -> None:
-        self.hyper[g] = spec
+    def set_hyper(self, g: int, rows: Tuple[HyperRow, ...]) -> None:
+        """Hyper-parameter rows of bucket g (sorted by ``end``, covering the bucket); allocates the state they need."""
+        self.hyper[g] = rows
+        for kind in self.family.shard_kinds(rows):
+            self.ensure_state(g, kind)
 
     def launches(self) -> int:
         return 0
@@ -169,9 +116,9 @@ class _BackendBase:
 class NativeBackend(_BackendBase):
     steal_grads = True
 
-    def __init__(self, comm, plan: BucketPlan, rank: int, world: int, device: torch.device,
+    def __init__(self, comm, family, plan: BucketPlan, rank: int, world: int, device: torch.device,
                  grad_comm_dtype: Optional[torch.dtype] = None):
-        super().__init__(plan, rank, world, device, grad_comm_dtype)
+        super().__init__(family, plan, rank, world, device, grad_comm_dtype)
         C = ops.require_native()
         self.C = C
         self.comm = comm
@@ -212,18 +159,15 @@ class NativeBackend(_BackendBase):
         for i in (range(len(self.where)) if g is None else (g,)):
             bs, li = self.where[i]
             if self.grad_shard[i] is not None:
-                bs.set_shards(li, self.grad_shard[i], self.mom_shard[i], self.master_shard[i], self.var_shard[i],
-                              self.gavg_shard[i])
+                sh = self.shards[i]
+                bs.set_shards(li, self.grad_shard[i], sh.get("mom"), sh.get("master"), sh.get("var"), sh.get("gavg"))
 
-    def set_hyper(self, g, spec: HyperSpec):
-        if self.hyper[g] == spec:
+    def set_hyper(self, g, rows):
+        if self.hyper[g] == rows:
             return
-        self.hyper[g] = spec
-        self._ensure_state(g, spec)
+        super().set_hyper(g, rows)
         bs, li = self.where[g]
-        bs.set_hyper(li, [s[0] for s in spec.segs], [s[1] for s in spec.segs], [s[2] for s in spec.segs],
-                     [s[3] for s in spec.segs], [s[4] for s in spec.segs], [int(s[5]) for s in spec.segs],
-                     [int(s[6]) for s in spec.segs], [s[7] for s in spec.segs], [s[8] for s in spec.segs])
+        bs.set_hyper(li, *(list(col) for col in zip(*rows)))    # one list per HyperRow field
 
     def set_step(self, t: int):
         for i, (bs, li) in enumerate(self.where):
@@ -299,9 +243,9 @@ class NativeBackend(_BackendBase):
 class TorchBackend(_BackendBase):
     steal_grads = False
 
-    def __init__(self, group, plan: BucketPlan, rank: int, world: int, device: torch.device,
+    def __init__(self, group, family, plan: BucketPlan, rank: int, world: int, device: torch.device,
                  grad_comm_dtype: Optional[torch.dtype] = None):
-        super().__init__(plan, rank, world, device, grad_comm_dtype)
+        super().__init__(family, plan, rank, world, device, grad_comm_dtype)
         self.group = group
         self.cuda = device.type == "cuda"
         self._pbuf = [torch.zeros(b.padded_numel, dtype=b.dtype, device=device) for b in plan.buckets]
@@ -320,10 +264,6 @@ class TorchBackend(_BackendBase):
 
     def grad_buffer(self, g):
         return self._gbuf[g]
-
-    def set_hyper(self, g, spec: HyperSpec):
-        self.hyper[g] = spec
-        self._ensure_state(g, spec)
 
     def set_step(self, t: int):
         self._t = int(t)
@@ -352,7 +292,7 @@ class TorchBackend(_BackendBase):
     def _clip_decide(self):
         """``torch.nn.utils.clip_grad_norm_`` over the averaged gradient: after the reduce-scatters every rank holds 1/P
         of it exactly once, so the norm is one pass over the fp32 shards plus a one-element all-reduce.  The
-        coefficient is applied in the update (``_sgd_shard``).  Eager steps only."""
+        coefficient is applied in the update (``_update_shard``).  Eager steps only."""
         if self.cuda and torch.cuda.is_current_stream_capturing():
             raise RuntimeError("norm_clip is not supported inside a CUDA-graph capture on the nccl backend")
         shards = [s for s in self.grad_shard if s is not None]
@@ -392,73 +332,28 @@ class TorchBackend(_BackendBase):
         self._n_launch += 3
 
     @torch.no_grad()
-    def _sgd_shard(self, g, first_step):
+    def _update_shard(self, g, first_step):
         if self.amp is not None:
             if self._skip:
                 return
             first_step = self._t == 0             # counts applied updates only
         b = self.plan.buckets[g]
         lo, hi = self.rank * b.shard_numel, (self.rank + 1) * b.shard_numel
-        master = self.master_shard[g]
+        master = self.shards[g].get("master")
         start = 0
-        for (end, lr, wd, mom, damp, nesterov, opt, beta2, eps) in self.hyper[g].segs:
-            a, z = max(start, lo), min(end, hi)
-            start = end
+        for row in self.hyper[g]:
+            a, z = max(start, lo), min(row.end, hi)
+            start = row.end
             if a >= z:
                 continue
-            if int(nesterov) & HYPER_SKIP and not bool(self.grad_shard[g][a - lo:z - lo].any()):
+            if row.flags & HYPER_SKIP and not bool(self.grad_shard[g][a - lo:z - lo].any()):
                 continue                          # no gradient on ANY rank this step: parameter and state stay as they are
-            centered = bool(int(nesterov) & HYPER_CENTERED)
-            nesterov = bool(int(nesterov) & HYPER_NESTEROV)
             sl = slice(a - lo, z - lo)
             p = master[sl] if master is not None else self._pbuf[g][a:z]
             d = self.grad_shard[g][sl]
             if self.clip is not None:
                 d = d * self.clip[2]
-            if opt == OPT_RMSPROP:
-                # torch.optim.RMSprop (_single_tensor_rmsprop); alpha is beta2, 1 - alpha is damp
-                if wd != 0:
-                    d = d.add(p, alpha=wd)
-                sq = self.var_shard[g][sl]
-                sq.mul_(beta2).addcmul_(d, d, value=damp)
-                if centered:
-                    ga = self.gavg_shard[g][sl]
-                    ga.lerp_(d, damp)
-                    avg = sq.addcmul(ga, ga, value=-1).sqrt_().add_(eps)
-                else:
-                    avg = sq.sqrt().add_(eps)
-                if mom > 0:
-                    buf = self.mom_shard[g][sl]
-                    buf.mul_(mom).addcdiv_(d, avg)
-                    p.add_(buf, alpha=-lr)
-                else:
-                    p.addcdiv_(d, avg, value=-lr)
-                self._n_launch += 5
-                continue
-            if opt != OPT_SGD:
-                t = self._t + 1
-                m, v = self.mom_shard[g][sl], self.var_shard[g][sl]
-                if opt == OPT_ADAM and wd != 0:
-                    d = d.add(p, alpha=wd)
-                m.mul_(mom).add_(d, alpha=1 - mom)
-                v.mul_(beta2).addcmul_(d, d, value=1 - beta2)
-                bc1, bc2 = 1 - mom ** t, 1 - beta2 ** t
-                if opt == OPT_ADAMW:
-                    p.mul_(1 - lr * wd)
-                p.addcdiv_(m, v.sqrt().div_(bc2 ** 0.5).add_(eps), value=-lr / bc1)
-                self._n_launch += 6
-                continue
-            if wd != 0:
-                d = d.add(p, alpha=wd)
-            if mom > 0:
-                buf = self.mom_shard[g][sl]
-                if first_step:
-                    buf.copy_(d)
-                else:
-                    buf.mul_(mom).add_(d, alpha=1 - damp)
-                d = d.add(buf, alpha=mom) if nesterov else buf
-            p.add_(d, alpha=-lr)
-            self._n_launch += 3
+            self._n_launch += self.family.update(row, p, d, self.shards[g], sl, first_step, self._t)
 
     def allgather_update(self, g, do_update=True, first_step=False, zero_grad=False):
         b = self.plan.buckets[g]
@@ -469,9 +364,9 @@ class TorchBackend(_BackendBase):
             if do_update and g == 0 and self.clip is not None:
                 self._clip_decide()
             if do_update:
-                self._sgd_shard(g, first_step)
-            if self.master_shard[g] is not None:
-                src = self.master_shard[g].to(b.dtype)
+                self._update_shard(g, first_step)
+            if "master" in self.shards[g]:
+                src = self.shards[g]["master"].to(b.dtype)
             else:
                 src = self._pbuf[g][lo:lo + b.shard_numel].clone()
             if self.world > 1:

@@ -24,7 +24,6 @@ GPU-first redesign (SURVEY.md §7, §9):
 """
 from __future__ import annotations
 
-import math
 import os
 from typing import Dict, List, Optional
 
@@ -32,9 +31,9 @@ import torch
 import torch.nn as nn
 
 from .. import runtime
-from .backends import (HYPER_CENTERED, HYPER_SKIP, OPT_ADAM, OPT_ADAMW, OPT_RMSPROP, OPT_SGD, HyperSpec, NativeBackend,
-                       TorchBackend)
+from .backends import SHARD_KINDS, NativeBackend, TorchBackend
 from .bucket import BucketPlan
+from .families import HYPER_SKIP, family_of
 
 import weakref
 
@@ -58,6 +57,8 @@ class DearEngine:
     def __init__(self, optimizer: torch.optim.Optimizer, model: nn.Module, *, threshold=THRESHOLD,
                  num_nearby_layers=NUM_NEARBY_LAYERS, exclude_parts: str = "", policy=None, verbose=True,
                  backward_passes_per_step: int = 1, grad_comm_dtype: Optional[torch.dtype] = None):
+        self.family = family_of(optimizer)         # parallel/families.py: SGD, Adam / AdamW or RMSprop
+        self.family.validate(optimizer.param_groups)
         if grad_comm_dtype not in (None, torch.float32, torch.bfloat16, torch.float16):
             raise ValueError("grad_comm_dtype must be None, torch.float32, torch.bfloat16 or torch.float16; got %r"
                              % (grad_comm_dtype,))
@@ -87,14 +88,6 @@ class DearEngine:
             raise ValueError("backward_passes_per_step must be >= 1")
         self.passes_per_step = int(backward_passes_per_step)   # gradient accumulation: reduce on the last pass only
         self._passes_seen = {}             # parameter -> backward passes since the last step()
-        if isinstance(optimizer, torch.optim.AdamW):
-            self.opt_kind = OPT_ADAMW
-        elif isinstance(optimizer, torch.optim.Adam):
-            self.opt_kind = OPT_ADAM
-        elif isinstance(optimizer, torch.optim.RMSprop):
-            self.opt_kind = OPT_RMSPROP
-        else:
-            self.opt_kind = OPT_SGD
         self._hooks = []
         self._closed = False
         self._wt = None                    # optional wait-time recorder (variants.WaitTimeBucketing)
@@ -104,14 +97,12 @@ class DearEngine:
         for p in model.parameters():
             if p.requires_grad and p.device.type != self.device.type:
                 raise RuntimeError("model parameters live on %s but the runtime device is %s" % (p.device, self.device))
-        # Adam / AdamW / RMSprop: updates a parameter did NOT take part in (no gradient on any rank).  torch.optim keeps
-        # the step count per parameter, the kernels keep one per bucket set: for Adam _refresh_hyper folds the difference
-        # into the parameter's hyper segment (see _adam_lag_adjust); RMSprop's math does not depend on the count, which
-        # only appears in its state_dict()
+        # families that count steps: updates a parameter did NOT take part in (no gradient on any rank).  torch.optim
+        # counts per parameter, the kernels per bucket set; Adam folds the difference into the parameter's row
+        # (Adam.lag_adjust), RMSprop only reports it in its state_dict()
         self._lag: Dict[nn.Parameter, int] = {}
-        # SGD with momentum AND dampening: torch initialises a parameter's momentum buffer with its first gradient
-        # (undampened); the kernels know one global "first step".  Parameters that start later get dampening 0 in
-        # their hyper segment for that one update (buf = m * 0 + 1 * g).  Filled below, empties after the first steps.
+        # SGD with momentum AND dampening (SGD.tracks_first_gradient): parameters still waiting for their first
+        # gradient, which gets a row with dampening 0 (buf = m * 0 + 1 * g).  Filled below, empties after the first steps.
         self._virgin = set()
         self.group_of: Dict[nn.Parameter, int] = {}
         for gi, grp in enumerate(optimizer.param_groups):
@@ -137,7 +128,7 @@ class DearEngine:
         if self.verbose:
             print("# of parameters: ", self.plan.num_parameters)
         self._check_plan_consistency()
-        if self.opt_kind == OPT_SGD and any(g.get("momentum", 0) != 0 and g.get("dampening", 0) != 0 for g in optimizer.param_groups):
+        if self.family.tracks_first_gradient(optimizer.param_groups):
             self._virgin = {s.param for s in self.plan.slots}
         self._build(initial=True)
         self._register_hooks()
@@ -186,9 +177,10 @@ class DearEngine:
 
     def _make_backend(self):
         if self.backend_name in ("b200", "emu"):
-            return NativeBackend(runtime.communicator(), self.plan, self.rank, self.world, self.device,
+            return NativeBackend(runtime.communicator(), self.family, self.plan, self.rank, self.world, self.device,
                                  self._grad_comm_dtype)
-        return TorchBackend(runtime.group(), self.plan, self.rank, self.world, self.device, self._grad_comm_dtype)
+        return TorchBackend(runtime.group(), self.family, self.plan, self.rank, self.world, self.device,
+                            self._grad_comm_dtype)
 
     @torch.no_grad()
     def _build(self, initial: bool, carry: Optional[dict] = None):
@@ -367,65 +359,49 @@ class DearEngine:
             self._next_rs -= 1
 
     # ------------------------------------------------------------------ hyper-parameters
-    @staticmethod
-    def _adam_lag_adjust(k, t: int, lag: int):
-        """Hyper-parameters that make the kernel's update with the GLOBAL step count ``t`` equal to Adam's update with
-        the parameter's own count ``s = t - lag`` (torch.optim counts steps per parameter and skips a parameter without
-        gradient):   lr/bc1(s) * m / (sqrt(v)/sqrt(bc2(s)) + eps)  ==  lr'/bc1(t) * m / (sqrt(v)/sqrt(bc2(t)) + eps')
-        with  r = sqrt(bc2(s)/bc2(t)),  eps' = eps r,  lr' = lr r bc1(t)/bc1(s);  AdamW's decoupled decay keeps
-        lr' wd' = lr wd."""
-        lr, wd, b1, damp, nest, opt, b2, eps = k
-        s = t - lag
-        r = math.sqrt((1.0 - b2 ** s) / (1.0 - b2 ** t)) if b2 < 1.0 else 1.0
-        lr2 = lr * r * ((1.0 - b1 ** t) / (1.0 - b1 ** s) if 0.0 < b1 < 1.0 else 1.0)
-        wd2 = wd * lr / lr2 if (opt == OPT_ADAMW and lr2 != 0.0) else wd
-        return (lr2, wd2, b1, damp, nest, opt, b2, eps * r)
-
     def _refresh_hyper(self):
-        key_all = self._hyper_key_now()
+        rows_all = self._hyper_key_now()
         t = self.num_updates + 1                     # the step count the kernels will use for the coming update
         for b in self.plan.buckets:
             absent = self._absent[b.index]
+            gone = set(absent)
             lags = None
-            if self.opt_kind in (OPT_ADAM, OPT_ADAMW) and self._lag:
+            if self.family.folds_lag and self._lag:
                 # (a parameter that sits this step out as well needs no correction now: no table churn for a branch
                 # that never runs)
-                gone_now = set(absent)
-                lags = tuple(0 if i in gone_now else self._lag.get(sl.param, 0) for i, sl in enumerate(b.slots))
+                lags = tuple(0 if i in gone else self._lag.get(sl.param, 0) for i, sl in enumerate(b.slots))
                 lags = (t, lags) if any(lags) else None
             fresh = ()
-            if self._virgin and self._mom_initialised and self.opt_kind == OPT_SGD:
-                gone_now = set(absent)
-                fresh = tuple(i for i, sl in enumerate(b.slots) if i not in gone_now and sl.param in self._virgin)
-            key = (key_all, absent, lags, fresh)
+            if self._virgin and self._mom_initialised:
+                fresh = tuple(i for i, sl in enumerate(b.slots) if i not in gone and sl.param in self._virgin)
+            key = (rows_all, absent, lags, fresh)
             if self._hyper_key[b.index] == key:
                 continue
-            segs = []
             if not absent and lags is None and not fresh:
-                for end, gi in self.plan.hyper_segments(b.index, self.group_of):
-                    segs.append((int(end),) + key_all[gi])
+                segs = self.plan.hyper_segments(b.index, self.group_of)
+                rows = [rows_all[gi]._replace(end=int(end)) for end, gi in segs]
             else:
                 # parameters that received no gradient on this rank carry HYPER_SKIP: where the reduced gradient is
                 # zero as well (absent on every rank) the update leaves them alone, like torch.optim skips
                 # ``p.grad is None`` (no weight decay, no momentum / moment decay)
-                gone, prev = set(absent), None
+                rows, prev = [], None
                 for i, sl in enumerate(b.slots):
                     gi, skip = self.group_of[sl.param], i in gone
                     lag = lags[1][i] if (lags is not None and not skip) else 0
                     end = b.slots[i + 1].start if i + 1 < len(b.slots) else b.padded_numel
-                    k = key_all[gi]
+                    row = rows_all[gi]
                     if lag and t - lag >= 1:
-                        k = self._adam_lag_adjust(k, t, lag)
+                        row = self.family.lag_adjust(row, t, lag)
                     first_own = i in fresh
                     if first_own:
-                        k = k[:3] + (0.0,) + k[4:]          # this parameter's first gradient: buf = g
-                    seg = (int(end),) + k[:4] + (int(k[4]) | (HYPER_SKIP if skip else 0),) + k[5:]
+                        row = row._replace(dampening=0.0)    # this parameter's first gradient: buf = g
+                    row = row._replace(end=int(end), flags=row.flags | (HYPER_SKIP if skip else 0))
                     if prev == (gi, skip, lag, first_own) and not lag:
-                        segs[-1] = seg
+                        rows[-1] = row
                     else:
-                        segs.append(seg)
+                        rows.append(row)
                     prev = (gi, skip, lag, first_own)
-            self.backend.set_hyper(b.index, HyperSpec(segs))
+            self.backend.set_hyper(b.index, tuple(rows))
             self._hyper_key[b.index] = key
 
     def freeze_hyper(self):
@@ -495,24 +471,8 @@ class DearEngine:
         return frozen if frozen is not None else self._hyper_key_live()
 
     def _hyper_key_live(self):
-        """Per param group: (lr, wd, momentum|beta1, dampening, nesterov, opt, beta2, eps).  RMSprop: (lr, wd,
-        momentum, 1 - alpha, HYPER_CENTERED if centered, OPT_RMSPROP, alpha, eps)."""
-        keys = []
-        for g in self.opt.param_groups:
-            if self.opt_kind == OPT_SGD:
-                keys.append((float(g["lr"]), float(g.get("weight_decay", 0.0)), float(g.get("momentum", 0.0)),
-                             float(g.get("dampening", 0.0)), bool(g.get("nesterov", False)), OPT_SGD, 0.0, 0.0))
-            elif self.opt_kind == OPT_RMSPROP:
-                alpha = float(g["alpha"])
-                # 1 - alpha is formed in double and rounded once, like the Python scalar torch hands to its kernels
-                keys.append((float(g["lr"]), float(g.get("weight_decay", 0.0)), float(g.get("momentum", 0.0)),
-                             1.0 - alpha, HYPER_CENTERED if g.get("centered", False) else 0, OPT_RMSPROP, alpha,
-                             float(g["eps"])))
-            else:
-                b1, b2 = g["betas"]
-                keys.append((float(g["lr"]), float(g.get("weight_decay", 0.0)), float(b1), 0.0, False, self.opt_kind,
-                             float(b2), float(g["eps"])))
-        return tuple(keys)
+        """Per param group: its HyperRow (``end`` 0)."""
+        return tuple(self.family.row(g) for g in self.opt.param_groups)
 
     def hyper_changed(self) -> bool:
         key = self._hyper_key_now()
@@ -620,18 +580,13 @@ class DearEngine:
             self._any_pending = True
             self._mom_initialised = True
             self.num_updates += 1
-            if self._virgin:
-                for g in range(nb):
-                    gone = set(self._absent[g])
-                    for i, sl in enumerate(self.plan.buckets[g].slots):
-                        if i not in gone:
-                            self._virgin.discard(sl.param)
-            if self.opt_kind != OPT_SGD:
-                for g in range(nb):
-                    if self._absent[g]:
-                        slots = self.plan.buckets[g].slots
-                        for i in self._absent[g]:
-                            self._lag[slots[i].param] = self._lag.get(slots[i].param, 0) + 1
+            for g in range(nb):
+                slots, absent = self.plan.buckets[g].slots, self._absent[g]
+                if self._virgin:
+                    self._virgin.difference_update(sl.param for i, sl in enumerate(slots) if i not in absent)
+                if self.family.counts_steps:
+                    for i in absent:
+                        self._lag[slots[i].param] = self._lag.get(slots[i].param, 0) + 1
         else:
             # time-breakdown mode (no all-gather): peers may still be pulling from this rank's
             # gradient buckets, so rendezvous on the device before the next backward reuses them
@@ -703,20 +658,15 @@ class DearEngine:
 
     @torch.no_grad()
     def _gather_state(self) -> dict:
-        """Full (un-sharded) optimizer state per parameter name: momentum and fp32 master."""
+        """Full (un-sharded) optimizer state per shard kind and parameter name (see ``_BackendBase.shards``)."""
         from ..utils.checkpoint import gather_sharded
-        out = {"momentum": {}, "master": {}, "var": {}, "gavg": {}, "mom_init": self._mom_initialised,
-               "num_updates": self.num_updates}
+        out = dict({kind: {} for kind in SHARD_KINDS}, mom_init=self._mom_initialised, num_updates=self.num_updates)
         if self.amp is not None:
             # skipped steps applied nothing: the device count of applied updates is the step count of the new buckets
             applied = self.read_scaler()["applied"]
             out.update(num_updates=applied, mom_init=applied > 0)
         for b in self.plan.buckets:
-            g = b.index
-            for kind, shard in (("momentum", self.backend.mom_shard[g]), ("master", self.backend.master_shard[g]),
-                                ("var", self.backend.var_shard[g]), ("gavg", self.backend.gavg_shard[g])):
-                if shard is None:
-                    continue
+            for kind, shard in self.backend.shards[b.index].items():
                 full = gather_sharded(shard, self.world)
                 for s in b.slots:
                     out[kind][s.name] = full[s.start:s.end].clone()
@@ -726,33 +676,20 @@ class DearEngine:
     def _restore_state(self, carry: dict):
         be = self.backend
         self._mom_initialised = bool(carry.get("mom_init", False))
-
         self.num_updates = int(carry.get("num_updates", self.num_updates))
         for b in self.plan.buckets:
             g = b.index
             lo, hi = self.rank * b.shard_numel, (self.rank + 1) * b.shard_numel
-            for kind in ("momentum", "master", "var", "gavg"):
+            for kind in SHARD_KINDS:
                 vals = carry.get(kind, {})
                 if not any(s.name in vals for s in b.slots):
                     continue
-                if kind == "momentum":
-                    be.ensure_momentum(g)
-                    shard = be.mom_shard[g]
-                elif kind == "var":
-                    be.ensure_var(g)
-                    shard = be.var_shard[g]
-                elif kind == "gavg":
-                    be.ensure_grad_avg(g)
-                    shard = be.gavg_shard[g]
-                else:
-                    shard = be.master_shard[g]
-                    if shard is None:
-                        continue
+                shard = be.shards[g].get(kind) if kind == "master" else be.ensure_state(g, kind)
+                if shard is None:           # (a master copy exists for low-precision buckets only)
+                    continue
                 for s in b.slots:
-                    if s.name not in vals:
-                        continue
                     a, z = max(s.start, lo), min(s.end, hi)
-                    if a < z:
+                    if s.name in vals and a < z:
                         shard[a - lo:z - lo].copy_(vals[s.name].reshape(-1)[a - s.start:z - s.start])
 
     def rebucket(self, policy):
@@ -798,24 +735,6 @@ class _DistributedOptimizer(torch.optim.Optimizer):
     def __init__(self, params, model, threshold=THRESHOLD, num_nearby_layers=NUM_NEARBY_LAYERS,
                  exclude_parts="", policy=None, verbose=True, backward_passes_per_step=1, grad_comm_dtype=None):
         super(self.__class__, self).__init__(params)
-        if not isinstance(self, (torch.optim.SGD, torch.optim.Adam, torch.optim.AdamW, torch.optim.RMSprop)):
-            raise TypeError(
-                "the decoupled all-reduce fuses the parameter update into the all-gather kernel; supported: "
-                "torch.optim.SGD (the reference's only DeAR optimizer, dear/dear_dopt.py:310-336), Adam, AdamW and "
-                "RMSprop; got %s. Use parallel.baselines for other optimizers." % type(self).__mro__[1].__name__)
-        if isinstance(self, torch.optim.RMSprop):
-            for g in self.param_groups:
-                for k in ("maximize", "capturable", "differentiable"):
-                    if g.get(k, False):
-                        raise ValueError("RMSprop with %s=True is not supported by the fused update" % k)
-                if isinstance(g["lr"], torch.Tensor):
-                    raise ValueError("RMSprop with a tensor lr is not supported by the fused update (pass a float)")
-        for g in self.param_groups:
-            if g.get("amsgrad", False) or g.get("capturable", False) or g.get("differentiable", False):
-                raise ValueError("amsgrad / capturable / differentiable Adam variants are not supported")
-        for g in self.param_groups:
-            if g.get("maximize", False):
-                raise ValueError("maximize=True is not supported")
         self._dear = DearEngine(self, model, threshold=threshold, num_nearby_layers=num_nearby_layers,
                                 exclude_parts=exclude_parts, policy=policy, verbose=verbose,
                                 backward_passes_per_step=backward_passes_per_step, grad_comm_dtype=grad_comm_dtype)
